@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- G+D training-step throughput (images/sec) at 256^2, batch 32 per GPU: BASELINE.json's metric on
-configs[2] ("full G+D train step (R1 + path-length reg) 256x256 bs32, synthetic FFHQ + FLAME, 1xB200").
+configs[2] ("full G+D train step (R1 + path-length reg) 256x256 bs32, synthetic FFHQ + FLAME"), on H100 (sm_90a).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-ppl]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-ppl] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -16,12 +16,12 @@ weights are random-initialised as the reference's constructors do.
   e2e          same loop, but every step copies that step's inputs from PINNED HOST memory and reads the two loss
                scalars back (the call a user of train.py makes: host batch in, losses out).
   precision    --precision bf16x3 (default, the headline): the error-compensated tensor-core contraction, the mode that
-               holds BASELINE.json's 1e-3 bar end to end (tests/test_models_gpu.py); the same step in plain kind::tf32
+               holds BASELINE.json's 1e-3 bar end to end (tests/test_models_gpu.py); the same step in plain tf32
                (faster, ~1e-3 forward / 1e-2 R1 deviation) is measured too and reported under "tf32_mode".
-  roofline     the dominant kernel = the tcgen05 implicit-GEMM convolution (conv_tc_kernel): algorithmic FLOPs of
-               every launch / its CUDA-event duration.  Peak: bf16x3 issues three kind::f16 MMAs per algorithmic MAC, so
-               its ceiling is MEASURED_PEAKS.json's sustained bf16 figure / 3; tf32: the cuBLAS TF32 GEMM rate measured
-               on this pool with the same protocol (profiles/r02_tf32_peak.json, tools/measure_tf32_peak.py).
+  roofline     the dominant kernel = the wgmma implicit-GEMM convolution (conv_tc_kernel): algorithmic FLOPs of
+               every launch / its CUDA-event duration.  Peak: NVIDIA's H100 SXM data-sheet dense rates (700 W card):
+               bf16x3 issues three bf16 MMAs per algorithmic MAC, so its ceiling is 989 TFLOP/s / 3; tf32: 495 TFLOP/s.
+               A power-capped card runs lower clocks; "clocks" in the line records what the card ran at.
   cpu_baseline the REFERENCE ITSELF on the host cores: its unmodified train() (train.py:80-252) over its own model / loss
                modules (build-time extract oracle/_ref/pyref, oracle/ref_import.py), fp32, all usable threads, on a bounded
                sample: batch 1, one R1 iteration and one plain iteration combined with the loop's 1/16 R1 share (~1 min;
@@ -30,6 +30,8 @@ weights are random-initialised as the reference's constructors do.
   --impl reference   times only that CPU arm (plus a warm-up iteration), rank 0 only.
   extras       BASELINE.json configs[1] (generator forward 256^2 bs16) and configs[3] (FLAME-topology texture+normal
                rasterisation 256^2 bs64, forward and forward+backward, with its HBM roofline fraction).
+  --dump-outputs DIR   the last timed step's losses and a seeded sample of the updated weights as DIR/<name>.npy
+               (dump_outputs); inputs and weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -49,6 +51,9 @@ import torch  # noqa: E402
 
 METRIC = "G+D train step images/sec @256x256 bs32/GPU"
 RES, BATCH, VOCAB = 256, 32, 70_000
+# NVIDIA H100 SXM data sheet (700 W): dense BF16 and TF32 tensor rates, HBM3 bandwidth
+H100_BF16_TFLOPS, H100_TF32_TFLOPS, H100_HBM_GBS = 989.4, 494.7, 3350.0
+DUMP_SAMPLE = 1 << 20
 
 
 _REAL_STDOUT = None
@@ -83,7 +88,25 @@ def parse():
     ap.add_argument("--no-other-precision", action="store_true", help="skip the extra measurement in the other precision mode")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[1] / configs[3] side measurements")
     ap.add_argument("--no-gpu-reference", action="store_true", help="skip timing the reference's own modules on this GPU (extra)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the losses and a seeded sample of the updated weights of the last timed step as DIR/<name>.npy")
     return ap.parse_args()
+
+
+def dump_outputs(path, losses, trainer):
+    """The result of the last timed step: the (d_loss, g_loss) pair train_iteration returns, and the weights that step left in
+    the three networks -- all of them when small, else the same sample of positions on every run (a permutation seeded with 0 of
+    the concatenated parameters, first DUMP_SAMPLE positions in ascending order; <= 13 MB in all)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, "d_loss.npy"), np.array([float(losses[0])], dtype=np.float64))
+    np.save(os.path.join(path, "g_loss.npy"), np.array([float(losses[1])], dtype=np.float64))
+    for name, net in (("generator", trainer.generator), ("discriminator", trainer.discriminator), ("g_running", trainer.g_running)):
+        flat = torch.cat([p.detach().reshape(-1).float() for p in net.parameters()])
+        if flat.numel() > DUMP_SAMPLE:
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(path, f"{name}_weights.npy"), flat.cpu().numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------------ clocks
@@ -226,7 +249,7 @@ def cpu_arm_reference(batch, warm_up, vocab=1000):
 
 def reference_on_gpu(batch=8, vocab=1000):
     """EXTRA, not the baseline of the contract: the reference's own modules and unmodified train() on THIS GPU through stock
-    PyTorch / cuDNN (what a user of the reference gets on a B200 today), 1 warm-up + 2 timed plain iterations at a reduced
+    PyTorch / cuDNN (what a user of the reference gets on this GPU today), 1 warm-up + 2 timed plain iterations at a reduced
     batch (its per-sample weight tensors and unfused upfirdn2d make batch 32 slow to autotune).  torch's stock precision flags (cuDNN convolutions may use TF32, matmuls fp32)."""
     from oracle import ref_import, ref_train_runner
     if not ref_import.available() or not torch.cuda.is_available():
@@ -327,11 +350,7 @@ def side_measurements(dev, trainer, resident):
     ms_fb = timeit(fwd_bwd)
     fwd_bytes = 3 * F * 36 + h * w * (4 + 4 + 12 + 12)                  # SURVEY 8d, texture+normal: 3.96 MB / image
     bwd_bytes = h * w * (12 + 12 + 4) + 3 * F * 36 + 3 * F * 36
-    hbm = 6487.4
-    try:
-        hbm = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
-    except (OSError, KeyError):
-        pass
+    hbm = H100_HBM_GBS
     out["config3_rasterize_texture_normal_256_bs64"] = {
         "renders_per_s_fwd": b / ms_f * 1e3, "renders_per_s_fwd_bwd": b / ms_fb * 1e3, "fwd_ms": ms_f, "fwd_bwd_ms": ms_fb,
         "roofline": {"bound": "hbm", "achieved": b * fwd_bytes / ms_f / 1e6, "peak": hbm, "unit": "GB/s",
@@ -379,6 +398,8 @@ def main():
     h2d = sum(t.numel() * t.element_size() for t in host[0])
     # R1 must fall inside every timed window: start the iteration counter so that the window contains
     # ceil(K/16) penalty iterations, the same share as in the reference's loop.
+    last = [None]
+
     def run(n, e2e):
         out = None
         for s in range(n):
@@ -393,6 +414,7 @@ def main():
             out = trainer.train_iteration(real, cond, idx, flm if trainer.interp_tex_loss is not None else None)
             if e2e:
                 out = (out[0].item(), out[1].item())      # device -> host read of the step's result
+        last[0] = out
         return out
 
     def barrier():
@@ -445,6 +467,8 @@ def main():
     ms = timed(args.steps, False)
     if cuprof:
         torch.cuda.profiler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0], trainer)
     launches = _lib.launch_count() - launches0 + trainer.replayed_launches
     prof = ops.PROFILE
     ops.PROFILE = None
@@ -453,12 +477,21 @@ def main():
     if use_graph:
         # graph replays cannot carry per-launch events: time the same kernels in a separate eager pass of the same steps
         # (all ranks run it -- it contains the gradient all-reduces -- only rank 0 records events)
-        saved, trainer._graphs = trainer._graphs, None
+        # the captured graphs' private memory pools and an eager iteration's activations do not fit in 80 GB together:
+        # release the graphs for this pass and capture them again afterwards
+        trainer._graphs = None
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()
         ops.PROFILE = [] if rank == 0 else None
         timed(min(args.steps, 4), False)
         prof = ops.PROFILE
         ops.PROFILE = None
-        trainer._graphs = saved
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()
+        trainer.capture(B, RES)
+        trainer.iteration = 14
+        run(2, False)
+        barrier()
         prof_note = ("per-launch CUDA events in a separate eager pass of %d steps after the timed region (CUDA-graph replays "
                      "cannot carry events; same kernels, same shapes)" % min(args.steps, 4))
     value = world * B * args.steps / (ms / 1000.0)
@@ -569,42 +602,23 @@ def main():
         tot_ms = sum(a.elapsed_time(b) for a, b, _, _ in prof)
         tot_fl = sum(f for _, _, f, _ in prof)
         prof_steps = min(args.steps, 4) if use_graph else args.steps
-        peaks, tf32pk = {}, {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except OSError:
-            pass
-        try:
-            tf32pk = json.load(open(os.path.join(ROOT, "profiles", "r02_tf32_peak.json")))
-        except OSError:
-            pass
-        bf16 = peaks.get("bf16_tflops_sustained")
         if args.precision == "bf16x3":
-            # three kind::f16 (bf16) MMAs per algorithmic multiply-add: the ceiling for ALGORITHMIC flops is bf16 peak / 3
-            peak = (bf16 if bf16 else 1400.0) / 3
-            peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained / 3 (bf16x3 issues hi*hi + hi*lo + lo*hi: three bf16 MMAs per "
-                        "algorithmic multiply-add)") if bf16 else "fallback 1.4 PFLOP/s sustained bf16 / 3"
+            # three bf16 MMAs per algorithmic multiply-add: the ceiling for ALGORITHMIC flops is the bf16 peak / 3
+            peak = H100_BF16_TFLOPS / 3
+            peak_src = ("H100 SXM data sheet, dense BF16 989 TFLOP/s at 700 W, / 3 (bf16x3 issues hi*hi + hi*lo + lo*hi: three "
+                        "bf16 MMAs per algorithmic multiply-add)")
         else:
-            t32 = tf32pk.get("tf32_tflops_sustained")
-            peak = t32 if t32 else (bf16 / 2 if bf16 else 700.0)
-            peak_src = ("profiles/r02_tf32_peak.json tf32_tflops_sustained (cuBLAS fp32 GEMM with TF32 tensor cores, 8192^3, 4 s "
-                        "back to back, measured on this pool with MEASURED_PEAKS.json's protocol)") if t32 else \
-                       "MEASURED_PEAKS.json bf16_tflops_sustained / 2"
+            peak = H100_TF32_TFLOPS
+            peak_src = "H100 SXM data sheet, dense TF32 495 TFLOP/s at 700 W"
         ach_all = tot_fl / (tot_ms * 1e-3) / 1e12 if tot_ms > 0 else 0.0
         ns = [(a.elapsed_time(b), f) for a, b, f, tag in prof if tag == "northstar"]
         # dominant kernel instance: conv_tc_kernel<128> on the north-star layer (B,128,256,256)->128, 3x3:
         # algorithmic FLOPs per launch = 2*9*128*128 per output pixel * 32*256*256 pixels = 618.5 GFLOP
         ach = (sum(f for _, f in ns) / (sum(t for t, _ in ns) * 1e-3) / 1e12) if ns else ach_all
-        traffic = None
-        try:    # DRAM bytes per launch of that kernel from the committed `ncu --set full` capture (profiles/)
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-            traffic = tj["conv_tc_northstar_dram_bytes_per_launch"][args.precision]
-        except (OSError, KeyError, ValueError, TypeError):
-            pass
-        kname = ("conv_tc_kernel<128, X3> (tcgen05 kind::f16, bf16x3 error-compensated implicit GEMM)" if args.precision == "bf16x3"
-                 else "conv_tc_kernel<128> (tcgen05 kind::tf32 implicit GEMM)")
+        kname = ("conv_tc_kernel<128, X3> (wgmma bf16, bf16x3 error-compensated implicit GEMM)" if args.precision == "bf16x3"
+                 else "conv_tc_kernel<128> (wgmma tf32 implicit GEMM)")
         roof = {"bound": "tensor", "kernel": kname + " on the north-star layer ModulatedConv2d 128->128 3x3 @256x256, batch 32",
-                "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
+                "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
                 "algorithmic_flops_per_launch": 2.0 * 9 * 128 * 128 * 32 * 256 * 256,
                 "algorithmic_hbm_bytes_per_launch": 2 * 32 * 256 * 256 * 128 * 4 + 9 * 128 * 128 * 4,
                 "launches_of_this_shape": len(ns), "avg_launch_ms": (sum(t for t, _ in ns) / len(ns)) if ns else None,
@@ -633,7 +647,7 @@ def main():
             "config": {"workload": "train_step_256_bs32: StyledGenerator(70000 ids) + Discriminator(256, 9ch), D step + G step, "
                                    "Adam, EMA, R1 every 16th iteration" + ("" if args.no_ppl else ", path-length reg every iteration"),
                        "global_batch": B * world, "resolution": RES, "parallelism": f"dp{world}", "cuda_graph": graph_note,
-                       "l2_policy": "inputs (4 x 75.5 MB batches, 1+ GB activations per layer) exceed the 126 MB L2"},
+                       "l2_policy": "inputs (4 x 75.5 MB batches, 1+ GB activations per layer) exceed the 50 MB L2"},
             "clocks": clocks, "gpu_launches": launches, "e2e": e2e, "roofline": roof, "cpu_baseline": cb,
             "same_step_without_path_length_reg": extra_no_ppl,
             ("tf32_mode" if args.precision == "bf16x3" else "bf16x3_mode"): other_mode,

@@ -1,4 +1,4 @@
-"""gif_b200 -- B200-native (sm_100a) implementation of GIF's data-parallel hot path.
+"""gif_b200 -- H100-native (sm_90a) implementation of GIF's data-parallel hot path.
 
 * ``gif_b200.model.stylegan2_common_layers`` / ``stg2_generator`` / ``stg2_discriminator``: drop-in operator and
   model classes (reference API, reference state_dict keys).

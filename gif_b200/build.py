@@ -1,6 +1,6 @@
-"""Builds gif_b200/libgifb200.so (hand-written CUDA for sm_100a + the C ABI of include/gifb200.h) with nvcc.
+"""Builds gif_b200/libgifb200.so (hand-written CUDA for sm_90a + the C ABI of include/gifb200.h) with nvcc.
 
-In-tree build: the .so lands next to this file so that it travels to the GPU box with the gpurun snapshot.
+In-tree build: the .so lands next to this file, so the package is importable from the source tree.
 ``python -m gif_b200.build`` or ``__graft_entry__.build()``.
 """
 import hashlib
@@ -15,7 +15,7 @@ OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libgifb200.so")
 SOURCES = ["elementwise.cu", "optim.cu", "upfirdn2d.cu", "sgemm.cu", "conv_simt.cu", "conv_tc.cu", "conv_wgrad_tc.cu", "conv_api.cu", "rasterize.cu", "render.cu", "flame.cu", "texture.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
          "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
 
@@ -29,11 +29,25 @@ def _stamp(path):
     return h.hexdigest()
 
 
+def _current():
+    """True when the library and every object exist and match the sources and flags (nothing to do, nothing written)."""
+    if not os.path.isfile(LIB):
+        return False
+    for src in SOURCES:
+        stamp_file = os.path.join(OBJ, src.replace(".cu", ".o")) + ".stamp"
+        if not os.path.isfile(stamp_file) or open(stamp_file).read() != _stamp(os.path.join(CSRC, src)):
+            return False
+    return True
+
+
 def build(verbose=False, force=False):
     """Incremental (content-hash stamps).  Safe under ``torchrun``: an exclusive file lock serialises concurrent builders
     (all ranks import the package at once), and every object / the library is written to a temporary name and renamed into
-    place, so a process that is not building never sees a half-written file."""
+    place, so a process that is not building never sees a half-written file.  A current build is left untouched without
+    taking the lock, so an already built tree may be read-only."""
     import fcntl
+    if not force and _current():
+        return LIB
     os.makedirs(OBJ, exist_ok=True)
     with open(os.path.join(OBJ, ".lock"), "w") as lock:
         fcntl.flock(lock, fcntl.LOCK_EX)

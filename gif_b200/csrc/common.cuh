@@ -1,4 +1,4 @@
-// Shared host/device helpers for libgifb200.so (sm_100a only).
+// Shared host/device helpers for libgifb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -38,7 +38,21 @@ inline int check_launch(const char* kernel) {
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 inline int cdiv(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
+
+// Deterministic cross-block sums.  A float atomicAdd per block adds the partial sums in whatever order the blocks finish, so
+// the result changes in its last bits from run to run, and an optimiser step turns that into visibly different weights.
+// Instead every block writes its partial sum to its own slot, part[slot * n + i]: slots_take points the kernel's output
+// pointer at a stream-ordered buffer (cudaMallocAsync, so it also works inside a CUDA graph), slots_reduce adds the slots
+// in slot order into the original output and frees the buffer.
+struct Slots {
+    float* part = nullptr;
+    float* out = nullptr;
+    int count = 0;
+    long long n = 0;
+};
+int slots_take(Slots& s, float*& out, int count, long long n, cudaStream_t st);
+int slots_reduce(Slots& s, cudaStream_t st);
 
 __device__ __forceinline__ float round_tf32(float v) {
     uint32_t r;

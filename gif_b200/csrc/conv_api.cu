@@ -1,4 +1,4 @@
-// gifb200_conv2d / gifb200_conv2d_wgrad: shape checks and dispatch between the tcgen05 and the SIMT kernels.
+// gifb200_conv2d / gifb200_conv2d_wgrad: shape checks and dispatch between the tensor-core and the SIMT kernels.
 #include "common.cuh"
 
 namespace gifb200 {
@@ -38,16 +38,16 @@ extern "C" int gifb200_conv2d(const float* x, const float* w, float* y, int B, i
     const bool prestaged = (impl & GIFB200_CONV_PRESTAGED) != 0;
     impl &= 0xF;
     GIFB200_REQUIRE(impl >= 0 && impl <= 3, GIFB200_E_SHAPE,
-                    "conv2d: impl must be 0 (auto), 1 (simt), 2 (tcgen05 tf32) or 3 (tcgen05 bf16x3 on split planes)");
+                    "conv2d: impl must be 0 (auto), 1 (simt), 2 (wgmma tf32) or 3 (wgmma bf16x3 on split planes)");
     const bool tc_ok = conv2d_tc_supported(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode);
-    if (impl >= 2 && !tc_ok) return fail(GIFB200_E_SHAPE, "conv2d: shape not supported by the tcgen05 path");
+    if (impl >= 2 && !tc_ok) return fail(GIFB200_E_SHAPE, "conv2d: shape not supported by the tensor-core path");
     if (impl != 1 && tc_ok)
         return conv2d_tc(x, w, y, B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, flip, transposed, epi, workspace, workspace_bytes, st,
                          impl == 3, prestaged);
     return conv2d_simt(x, w, y, B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, flip, transposed, epi, st);
 }
 
-// > 0 exactly when the tcgen05 path will be taken (split-K partial sums live in the workspace)
+// > 0 exactly when the tensor-core path will be taken (split-K partial sums live in the workspace)
 extern "C" size_t gifb200_conv2d_wgrad_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, int Wo, int Co, int k,
                                                        int mode, int impl) {
     if (impl == 1) return 0;
@@ -65,7 +65,7 @@ extern "C" int gifb200_conv2d_wgrad(const float* x, const float* gy, float* gw, 
                                     size_t workspace_bytes, gifb200_stream_t stream) {
     GIFB200_REQUIRE(impl >= 0 && impl <= 3, GIFB200_E_SHAPE, "conv2d_wgrad: impl must be 0, 1, 2 or 3");
     const bool tc_ok = conv2d_wgrad_tc_supported(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode);
-    if (impl >= 2 && !tc_ok) return fail(GIFB200_E_SHAPE, "conv2d_wgrad: shape not supported by the tcgen05 path");
+    if (impl >= 2 && !tc_ok) return fail(GIFB200_E_SHAPE, "conv2d_wgrad: shape not supported by the tensor-core path");
     if (impl != 1 && tc_ok)
         return conv2d_wgrad_tc(x, gy, gw, B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, flip, transposed, workspace,
                                workspace_bytes, static_cast<cudaStream_t>(stream), impl == 3);

@@ -1,6 +1,6 @@
 // SIMT fp32 implicit-GEMM convolution (forward / input-gradient for all three modes, and weight gradient).
 //
-// Role: (1) the exact-fp32 path for shapes the tcgen05 kernel does not take (Ci or Co not a multiple of 32/16:
+// Role: (1) the exact-fp32 path for shapes the tensor-core kernel does not take (Ci or Co not a multiple of 32/16:
 // the 9-channel D stem, the 6->12->24 NoiseInjection convs, ragged test shapes), (2) the on-GPU cross-check of the
 // tensor-core kernel.  Tiling: 64 output pixels x 64 output channels per CTA, K chunks of 16 input channels per
 // tap, 256 threads with 4x4 register micro-tiles.
@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const float* __restrict_
 //   S1: S = gy (Cs=Co), Bg = x (Cb=Ci), st=1, pad=k/2;   S2: S = gy, Bg = x, st=2, pad=0;
 //   T2: S = x (Cs=Ci), Bg = gy (Cb=Co), st=2, pad=0  (the roles of the two tensors swap).
 // The result is scattered into the physical weight layout through (stride_cs, stride_cb).  Split over pixels
-// (gridDim.z = T * splits) with fp32 atomics into the zero-initialised output.
+// (gridDim.z = T * splits): every split writes its own slot of a Slots buffer (common.cuh), added in split order.
 struct WgradParams {
     int B, Hs, Ws, Cs, Hb, Wb, Cb, k, st, pad, flip, splits;
     long long Ms;  // B*Hs*Ws
@@ -197,7 +197,7 @@ __global__ void __launch_bounds__(256) wgrad_simt_kernel(const float* __restrict
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int cb = cb0 + tn + j;
-            if (cb < p.Cb) atomicAdd(out + tt * p.stride_t + cs * p.stride_cs + cb * p.stride_cb, acc[i][j]);
+            if (cb < p.Cb) out[split * p.k * p.k * p.stride_t + tt * p.stride_t + cs * p.stride_cs + cb * p.stride_cb] = acc[i][j];
         }
     }
 }
@@ -266,9 +266,11 @@ int conv2d_wgrad_simt(const float* x, const float* gy, float* gw, int B, int Hi,
     if (splits < 1) splits = 1;
     if (splits * T > 65535) splits = 65535 / T;
     p.splits = static_cast<int>(splits);
+    Slots sl;
+    if (int rc2 = slots_take(sl, gw, p.splits, static_cast<long long>(T) * Co * Ci, st)) return rc2;
     wgrad_simt_kernel<<<dim3(gx, gy_, T * p.splits), 256, 0, st>>>(S, Bg, gw, p);
     GIFB200_LAUNCH_CHECK("wgrad_simt_kernel");
-    return GIFB200_OK;
+    return slots_reduce(sl, st);
 }
 
 }  // namespace gifb200

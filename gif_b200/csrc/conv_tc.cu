@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution for sm_100a (kind::tf32, fp32 accumulation in TMEM).
+// wgmma implicit-GEMM convolution for sm_90a (tf32 operands, fp32 accumulation in registers).
 //
 // GEMM view (per output "phase"):  D[site, o] = sum_{tap} sum_{i} A_tap[site, i] * W[tap][o][i]
 //   M = 128 sites per CTA (a wt x ht x nt box of the site grid (B, Hs, Ws)), N = BLOCK_N output channels,
@@ -10,21 +10,21 @@
 //     subset of the 9 taps, and write with output stride 2.
 //   * B operand: the tap-major weights [T][Co][Ci] staged once per call into the workspace (honouring flip /
 //     transposed, rounded to tf32), K-major, 128B swizzle.
-//   * Both operands are K-major SWIZZLE_128B; one tcgen05.mma.cta_group::1.kind::tf32 (M=128, N=BLOCK_N, K=8) per
-//     32-byte K slice, issued by one thread; accumulators live in TMEM (BLOCK_N columns).
-//   * Warp roles (256 threads): warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-7 epilogue
-//     (tcgen05.ld 32x32b -> registers -> 16-byte global stores, channels-last).
+//   * Both operands are K-major SWIZZLE_128B; each of two consumer warpgroups issues one wgmma.m64nNk8.tf32 (its 64 rows
+//     of the tile, N = BLOCK_N) per 32-byte K slice; accumulators live in registers (BLOCK_N / 2 per thread).
+//   * Warp roles (288 threads): warps 0-7 two consumer warpgroups (MMA + fused epilogue from registers, 8-byte global
+//     stores, channels-last), warp 8 TMA producer.
 //   * 3-stage smem ring (96 KB) so that two CTAs share an SM: one CTA's epilogue overlaps the other's main loop.
 //
-// Operand precision: kind::tf32 reads the upper 19 bits of each fp32 (truncation).  Callers hand in activations that
+// Operand precision: the tf32 MMA reads the upper 19 bits of each fp32 (truncation).  Callers hand in activations that
 // are already rounded to tf32 (gif_b200.ops rounds in the producing kernel), weights are rounded here, so the
 // truncation is exact and the contraction is an unbiased tf32 x tf32 -> fp32 product sum.
 //
 // X3 = true is the error-compensated mode ("bf16x3", gifb200_conv2d impl 3): operands arrive as two bf16 planes (hi, lo)
 // per tensor (gifb200_split_bf16; the weights are split while staging), a stage holds the hi and the lo tile of A and of B
 // as K-major SWIZZLE_64B tiles of 32 channels (128 rows x 64 B: the SAME number of bytes per stage as the fp32 tiles), and
-// each 16-channel slice issues three kind::f16 MMAs -- lo*hi, hi*lo, hi*hi -- into the one fp32 TMEM accumulator.
-// Everything else (tile walk, ring, double-buffered TMEM, epilogue) is shared with the tf32 kernel.
+// each 16-channel slice issues three bf16 wgmmas -- lo*hi, hi*lo, hi*hi -- into the one fp32 register accumulator.
+// Everything else (tile walk, ring, epilogue) is shared with the tf32 kernel.
 #include <cuda_bf16.h>
 
 #include "tc_common.cuh"
@@ -38,7 +38,8 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 32;                         // fp32 elements = 128 bytes = one swizzle row
 constexpr int kATileBytes = kBlockM * kBlockK * 4;  // 16 KB
 constexpr int kMaxTaps = 9;
-constexpr int kTcThreads = 384;   // warps 0-3: TMA / MMA / TMEM alloc / spare; warps 4-11: epilogue (2 per TMEM lane quarter)
+constexpr int kConsumerWarps = 8;                   // two warpgroups: rows 0-63 and 64-127 of the tile
+constexpr int kTcThreads = 32 * kConsumerWarps + 32;   // + one TMA producer warp
 
 struct TcParams {
     int B, Hs, Ws;          // site grid per image
@@ -57,7 +58,7 @@ struct TcParams {
     int in_sy;
     int ksplit;             // > 1: the K loop (taps x channel chunks) of every tile is cut into ksplit ranges, one tile each,
     float* part;            //      whose accumulators go to part[ks][...] (same indexing as y); splitk_reduce_kernel sums them
-    long long part_stride;  //      in a fixed order and applies the epilogue (small layers: 16 output tiles cannot fill 148 SMs)
+    long long part_stride;  //      in a fixed order and applies the epilogue (small layers: 16 output tiles cannot fill 132 SMs)
     ConvEpilogue epi;
 };
 
@@ -66,21 +67,14 @@ struct SmemLayout {
     static constexpr int kBTileBytes = BLOCK_N * kBlockK * 4;
     static constexpr int kStageBytes = kATileBytes + kBTileBytes;
     static constexpr int kBarrierOffset = kStages * kStageBytes;
-    static constexpr int kTotal = kBarrierOffset + 128;   // full[3], empty[3], tmem_full[2], tmem_empty[2], tmem ptr
+    static constexpr int kTotal = kBarrierOffset + 64;    // full[3], empty[3]
     static constexpr int kDynamic = kTotal + 1024;        // slack for manual 1024 B alignment
-    static constexpr int kTmemCols = 2 * BLOCK_N < 32 ? 32 : 2 * BLOCK_N;   // two accumulator buffers
 };
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 
 // Tile order: (output-channel block, phase) vary FASTEST, the site tile slowest, so that the CTAs running at the same
 // time read the same activation boxes and the re-reads (once per channel block, per phase, per tap) hit L2 instead of
-// DRAM.  (ncu on the phase-major order, T2 512->256 @64->129, B=32: 2.56 GB of DRAM reads for a 268 MB input, 4.7 TB/s,
-// i.e. memory-bound on re-reads.)  Phases have 4/2/2/1 taps; the phase a CTA gets is rotated from round to round
-// (rot = (mtile / rot_div) % nphase, a function of the site tile only, hence still a bijection) so every CTA sees all
-// phases equally often.
+// DRAM.  Phases have 4/2/2/1 taps; the phase a CTA gets is rotated from round to round (rot = (mtile / rot_div) % nphase,
+// a function of the site tile only, hence still a bijection) so every CTA sees all phases equally often.
 __device__ __forceinline__ void decode_tile(int tile, int nblocks, int nphase, int rot_div, int& mt, int& nblk, int& phase) {
     const int inner = nblocks * nphase;
     mt = tile / inner;
@@ -89,9 +83,10 @@ __device__ __forceinline__ void decode_tile(int tile, int nblocks, int nphase, i
     phase = nphase == 1 ? 0 : (rem / nblocks + mt / rot_div) % nphase;
 }
 
-// Persistent: gridDim.x CTAs (<= 2 per SM) walk the tile list (see decode_tile).
-// The smem ring and its phase bits run continuously across tiles; the TMEM accumulator is double buffered so the
-// epilogue of tile i overlaps the main loop of tile i+1 of the same CTA (and the second resident CTA fills the rest).
+// Persistent: gridDim.x CTAs (<= 2 per SM) walk the tile list (see decode_tile).  Warps 0-7 are two consumer warpgroups
+// (wgmma into register accumulators, then the fused epilogue straight from registers), warp 8 is the TMA producer.  The
+// smem ring and its phase bits run continuously across tiles; the second resident CTA overlaps its main loop with this
+// CTA's epilogue.
 template <int BLOCK_N, bool X3>
 __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_constant__ CUtensorMap map_a,
                                                          const __grid_constant__ CUtensorMap map_a2,
@@ -104,9 +99,6 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarrierOffset);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full_bar = empty_bar + kStages;        // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;         // [2]
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nblocks = p.Co / BLOCK_N;
@@ -114,34 +106,23 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
     const int rot_div = max(1, static_cast<int>(gridDim.x) / (nblocks * p.nphase));
     (void)mtiles;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kConsumerWarps && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         if (X3) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a2) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b2) : "memory");
         }
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full_bar[b], 1); mbar_init(&tmem_empty_bar[b], kTcThreads - 128); }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(L::kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         // ===================== TMA producer =====================
-        // Lane 0 owns the barriers.  In stride-2 mode the A tile is nt*ht separate row boxes (the parity view cannot be
-        // one box): the 32 lanes issue them in parallel -- at 9x9 / 17x17 inputs a stage is 32 / 16 row loads and a
-        // single issuing thread was the whole critical path (340 us for a 2.4 GFLOP layer).
+        // Lane 0 owns the barriers.  In stride-2 row mode the A tile is nt*ht separate row boxes (the parity view cannot be
+        // one box): the 32 lanes issue them in parallel.
         int stage = 0;
         uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -197,107 +178,88 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
                 if (++stage == kStages) { stage = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1 && lane == 0) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = X3 ? make_idesc_bf16(kBlockM, BLOCK_N) : make_idesc_tf32(kBlockM, BLOCK_N);
+    } else {
+        // ===================== consumers: wgmma main loop + epilogue =====================
+        const int wg = warp >> 2;                    // rows 64*wg .. 64*wg+63 of the tile
+        const int wq = warp & 3;
+        constexpr int kAcc = BLOCK_N / 2;
+        float acc[kAcc];
+        // the two rows (h = 0, 1) this thread holds in the accumulator fragment, and their place in the site box
+        int w_in[2], h_in[2], n_in[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            w_in[h] = r % p.wt; h_in[h] = (r / p.wt) % p.ht; n_in[h] = r / (p.wt * p.ht);
+        }
         int stage = 0;
         uint32_t ph = 0;
-        int local = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++local) {
-            int mt_, nblk_, phase;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            int mt, nblk, phase;
             const int ks = tile % p.ksplit;
-            decode_tile(tile / p.ksplit, nblocks, p.nphase, rot_div, mt_, nblk_, phase);
+            decode_tile(tile / p.ksplit, nblocks, p.nphase, rot_div, mt, nblk, phase);
             const int iters = p.phase_ntaps[phase] * kchunks;
             const int it0 = iters * ks / p.ksplit, it1 = iters * (ks + 1) / p.ksplit;
-            const int buf = local & 1;
-            mbar_wait(&tmem_empty_bar[buf], ((local >> 1) & 1) ^ 1);     // epilogue has drained this buffer
-            tcgen05_fence_after();
-            const uint32_t tmem_d = tmem_base + buf * BLOCK_N;
+            int prev = -1;
             for (int it = it0; it < it1; ++it) {
                 mbar_wait(&full_bar[stage], ph);
-                tcgen05_fence_after();
                 const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
+                wgmma_fence();
+                fence_regs<kAcc>(acc);
                 if (X3) {
                     // v = hi + lo per operand: acc += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (the 2^-18 lo*lo term is dropped);
-                    // small terms first.  UMMA_K = 16 bf16 = 32 bytes: two slices per 32-channel stage.
-                    const uint64_t ah = make_kmajor_sw64_desc(a_addr), al = make_kmajor_sw64_desc(a_addr + kATileBytes / 2);
+                    // small terms first.  K = 16 bf16 = 32 bytes: two slices per 32-channel stage.  A rows of 64 B.
+                    const uint32_t a_wg = a_addr + wg * 64 * 64;
+                    const uint64_t ah = make_kmajor_sw64_desc(a_wg), al = make_kmajor_sw64_desc(a_wg + kATileBytes / 2);
                     const uint64_t bh = make_kmajor_sw64_desc(a_addr + kATileBytes);
                     const uint64_t bl = make_kmajor_sw64_desc(a_addr + kATileBytes + L::kBTileBytes / 2);
 #pragma unroll
                     for (int k = 0; k < kBlockK / 16; ++k) {
-                        umma_bf16(tmem_d, al + 2 * k, bh + 2 * k, idesc, (it != it0) || k != 0);
-                        umma_bf16(tmem_d, ah + 2 * k, bl + 2 * k, idesc, 1);
-                        umma_bf16(tmem_d, ah + 2 * k, bh + 2 * k, idesc, 1);
+                        wgmma_bf16<BLOCK_N>(acc, al + 2 * k, bh + 2 * k, (it != it0) || k != 0, Trans<0>());
+                        wgmma_bf16<BLOCK_N>(acc, ah + 2 * k, bl + 2 * k, 1, Trans<0>());
+                        wgmma_bf16<BLOCK_N>(acc, ah + 2 * k, bh + 2 * k, 1, Trans<0>());
                     }
                 } else {
-                    const uint64_t adesc = make_kmajor_sw128_desc(a_addr);
+                    const uint64_t adesc = make_kmajor_sw128_desc(a_addr + wg * 64 * 128);
                     const uint64_t bdesc = make_kmajor_sw128_desc(a_addr + kATileBytes);
 #pragma unroll
-                    for (int k = 0; k < kBlockK / 8; ++k)   // UMMA_K = 8 tf32 = 32 bytes: advance the start address by 32 B (>>4 = 2)
-                        umma_tf32(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (it != it0) || k != 0);
+                    for (int k = 0; k < kBlockK / 8; ++k)   // K = 8 tf32 = 32 bytes: advance the start address by 32 B (>>4 = 2)
+                        wgmma_tf32<BLOCK_N>(acc, adesc + 2 * k, bdesc + 2 * k, (it != it0) || k != 0);
                 }
-                umma_commit(&empty_bar[stage]);          // frees the smem slot when these MMAs retire
+                wgmma_commit();
+                fence_regs<kAcc>(acc);
+                // keep this stage's MMAs in flight; the previous stage's have retired -> its smem slot is free
+                wgmma_wait<1>();
+                if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+                prev = stage;
                 if (++stage == kStages) { stage = 0; ph ^= 1; }
             }
-            umma_commit(&tmem_full_bar[buf]);            // accumulator complete
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int q = warp & 3;                      // TMEM lane quarter this warp may access (warp id mod 4)
-        const int half = (warp - 4) >> 2;            // which half of the tile's columns this warp drains
-        constexpr int kColsPerWarp = BLOCK_N >= 64 ? BLOCK_N / 2 : BLOCK_N;
-        const bool active = BLOCK_N >= 64 || half == 0;
-        const int r = q * 32 + lane;                 // tile row == TMEM lane
-        const int w_in = r % p.wt, h_in = (r / p.wt) % p.ht, n_in = r / (p.wt * p.ht);
-        int local = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++local) {
-            int mt, nblk, phase;
-            const int ks = tile % p.ksplit;
-            decode_tile(tile / p.ksplit, nblocks, p.nphase, rot_div, mt, nblk, phase);
+            wgmma_wait<0>();
+            fence_regs<kAcc>(acc);
+            if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+            // ---- epilogue: registers -> channels-last global (split-K: this split's partial buffer, epilogue deferred)
             int m = mt;
             const int tx = m % p.tiles_x; m /= p.tiles_x;
             const int ty = m % p.tiles_y; m /= p.tiles_y;
-            const int n = m * p.nt + n_in;
-            const int Y = (ty * p.ht + h_in) * p.oys + p.phase_oy0[phase], X = (tx * p.wt + w_in) * p.oxs + p.phase_ox0[phase];
-            const bool ok = active && n < p.B && Y < p.Ho && X < p.Wo;
-            const int col0 = (BLOCK_N >= 64 ? half * kColsPerWarp : 0);
-            float* dst = (p.ksplit > 1 ? p.part + ks * p.part_stride : y) +
-                         ((static_cast<long long>(n) * p.Ho + Y) * p.Wo + X) * p.Co + nblk * BLOCK_N + col0;
-            const int buf = local & 1;
-            mbar_wait(&tmem_full_bar[buf], (local >> 1) & 1);
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int c = 0; active && c < kColsPerWarp; c += 32) {
-                uint32_t v[32];
-                const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BLOCK_N + col0 + c;
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                      "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                      "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                      "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (ok) {
-                    if (p.epi.act && p.ksplit == 1) {      // split-K: the reduction pass applies the epilogue to the sum
-                        const int o0 = nblk * BLOCK_N + col0 + c;
+            float* base = p.ksplit > 1 ? p.part + ks * p.part_stride : y;
+            const int c0 = nblk * BLOCK_N + 2 * (lane & 3);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(apply_epilogue(p.epi, __uint_as_float(v[j]), o0 + j));
+            for (int h = 0; h < 2; ++h) {
+                const int n = m * p.nt + n_in[h];
+                const int Y = (ty * p.ht + h_in[h]) * p.oys + p.phase_oy0[phase], X = (tx * p.wt + w_in[h]) * p.oxs + p.phase_ox0[phase];
+                if (n < p.B && Y < p.Ho && X < p.Wo) {
+                    float* dst = base + ((static_cast<long long>(n) * p.Ho + Y) * p.Wo + X) * p.Co + c0;
+#pragma unroll
+                    for (int j = 0; j < BLOCK_N / 8; ++j) {
+                        float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                        if (p.epi.act && p.ksplit == 1) {      // split-K: the reduction pass applies the epilogue to the sum
+                            v.x = apply_epilogue(p.epi, v.x, c0 + 8 * j);
+                            v.y = apply_epilogue(p.epi, v.y, c0 + 8 * j + 1);
+                        }
+                        *reinterpret_cast<float2*>(dst + 8 * j) = v;
                     }
-#pragma unroll
-                    for (int j = 0; j < 32; j += 8) st_global_v8(dst + c + j, v + j);   // 32-byte stores: whole sectors
                 }
             }
-            tcgen05_fence_before();
-            mbar_arrive(&tmem_empty_bar[buf]);       // all 256 epilogue threads arrive -> buffer released to the MMA issuer
         }
-    }
-    __syncthreads();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(L::kTmemCols) : "memory");
     }
 }
 
@@ -344,7 +306,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
 }
 
 // K splits for a layer whose output tiles cannot fill the machine (4x4 / 8x8 layers at batch 32: 16-64 tiles, 144 pipeline
-// iterations each; the stride-2 9x9 layer ran at 10 TFLOP/s, bound by one CTA's TMA issue rate).  Stride-1 / stride-2 modes.
+// iterations each: otherwise one CTA's TMA issue rate bounds the layer).  Stride-1 / stride-2 modes.
 int pick_ksplit(long long tiles, int iters, int mode) {
     if (mode == 2 || tiles > kNumSMs / 2 || iters < 8) return 1;
     long long ks = (2LL * kNumSMs) / tiles;
@@ -587,8 +549,6 @@ int conv2d_tc(const float* x, const float* w, float* y, int B, int Hi, int Wi, i
     // not cover).  Row Y = 2*Hi only sees kernel row kh = 2 applied to input row Hi-1: a 1-D transposed convolution along x;
     // likewise the column along y with kw = 2.  Both run through the SAME tensor-core kernel on 1-row / 1-column views of
     // the input (two more launches of ~1/64 of the main work each); the single corner pixel is a dot product per (b, o).
-    // (Until round 1 this border was an fp32 SIMT strip kernel on an auxiliary stream: 0.35 ms per large layer, and it
-    // competed with the persistent tensor-core CTAs for SMs.)
     for (int edge = 0; edge < 2 && rc == GIFB200_OK; ++edge) {
         const bool row = edge == 0;
         TcParams q;

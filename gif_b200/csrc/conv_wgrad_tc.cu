@@ -1,17 +1,16 @@
-// tcgen05 weight-gradient kernel (kind::tf32): R[t][cs][cb] = sum_{pixels p} S[p][cs] * Bg[map(p,t)][cb]
+// Tensor-core weight-gradient kernel for sm_90a: R[t][cs][cb] = sum_{pixels p} S[p][cs] * Bg[map(p,t)][cb]
 //
 //   S  = "small-grid" tensor (B,Hs,Ws,Cs): the conv OUTPUT gradient for S1/S2, the conv INPUT for T2
 //   Bg = "big" tensor (B,Hb,Wb,Cb) read at map(p,t) = (y+kh-pad, x+kw-pad)  (S1)  or (2y+kh, 2x+kw)  (S2 / T2)
 //
-// GEMM view per CTA: M = 128 small channels, N = BLOCK_N big channels, K = pixels.  Both operands are
-// channels-last, i.e. MN-contiguous ("MN-major"): a TMA box (32 channels x P pixels) lands as P rows of 128 bytes.
-// For 32-bit MN-major operands the only legal UMMA shared-memory layout is SWIZZLE_128B_BASE32B (32-byte chunks
-// XOR-ed with the row index mod 4; cutlass sm100_common.inl:92) -- the TMA side is CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.
-// Descriptor: 4-row K atoms (SBO = 512 B between them), LBO = distance between 32-channel chunks.  One tcgen05.mma
-// (M=128, N=BLOCK_N, K=8 pixels) consumes two K atoms; the next 8 pixels are +1024 B.
+// GEMM view per CTA: M = 128 small channels, N = BLOCK_N (<= 64) big channels, K = pixels.  Both operands are
+// channels-last, i.e. MN-contiguous ("MN-major"): a TMA box (32 channels x P pixels) lands as P rows of 32 channels.
 // A CTA owns one kernel row kh and all KW taps of it: the S tile is loaded once per stage and multiplied with the KW
-// shifted Bg tiles into KW separate TMEM accumulators (KW*BLOCK_N <= 384 columns).  The pixel range is split across
-// CTAs (split-K); partial results are added into the zero-initialised output with fp32 atomics.
+// shifted Bg tiles into KW separate register accumulators.  The pixel range is split across CTAs (split-K); every split
+// writes its own slice of a partial buffer and wgrad_reduce_kernel sums the slices in a fixed order (deterministic).
+// Warps 0-7 consume, warp 8 is the TMA producer.
+//
+// tf32: wgmma takes 32-bit operands K-major only, so the MN-major fp32 tiles are read as mma.sync.m16n8k8 fragments.
 //
 // STACK variant (Cs == 32, stride-1 3x3: the zero-padded NoiseInjection convs): M = 128 cannot be filled with channels,
 // so the four 32-row chunks of the A tile hold the SAME 32 channels of S at three different row shifts (dy = +1, 0, -1;
@@ -20,8 +19,9 @@
 //
 // X3 = true ("bf16x3", gifb200_conv2d_wgrad impl 3): both operands arrive as two bf16 planes (hi, lo; gifb200_split_bf16).
 // 16-bit MN-major tiles of 32 channels use the canonical SWIZZLE_64B layout (rows of 64 bytes, 8-pixel K atoms of 512 B; TMA
-// side CU_TENSOR_MAP_SWIZZLE_64B); a stage holds the hi and the lo chunk set of each operand -- the SAME bytes as the fp32
-// tiles -- and every 16-pixel slice issues three kind::f16 MMAs (lo*hi, hi*lo, hi*hi) into the tap's fp32 TMEM accumulator.
+// side CU_TENSOR_MAP_SWIZZLE_64B), which wgmma reads transposed; a stage holds the hi and the lo chunk set of each operand --
+// the SAME bytes as the fp32 tiles -- and every 16-pixel slice issues three bf16 wgmmas (lo*hi, hi*lo, hi*hi) per
+// warpgroup into the tap's fp32 accumulator.
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -29,46 +29,33 @@
 namespace gifb200 {
 namespace {
 
-constexpr int kWgStages = 3;
+constexpr int kWgStages = 4;
 constexpr int kPix = 32;                       // pixels (GEMM K) per stage
 constexpr int kAChunks = 4;                    // M = 128 small channels
+constexpr int kWgConsumerWarps = 8;            // two warpgroups (X3: wgmma on rows 0-63 / 64-127) or 4 x 2 mma.sync warps
+constexpr int kWgThreads = 32 * kWgConsumerWarps + 32;   // + one TMA producer warp
 
 struct WgParams {
     int B, Hs, Ws, Cs, Hb, Wb, Cb;
     int k, pad, s2, flip;
-    int halo_bo;            // HALO: put the row phase of the tap's start address into the descriptor's base_offset field
     int pw;                 // pixels per TMA row load (min(Ws, 32)); rows per stage = 32 / pw
     int mr_s, mr_b;         // narrow images (pw < 32): the S / Bg tensor map's box spans ALL rows of a stage (by rows x bn images),
-                            // one TMA issue per chunk and tap instead of one per row (the 4x4 layers issued 256 loads per stage)
+                            // one TMA issue per chunk and tap instead of one per row
     long long units;        // number of 32-pixel units in the small grid
     int splits;
     long long stride_t, stride_cs, stride_cb;
     long long part_stride;   // floats per split in the partial buffer: T * Cs_total * Cb (layout [split][t][cs][cb])
 };
 
-// MN-major descriptor.  fp32: LayoutType::SWIZZLE_128B_BASE32B (1), 4-pixel K atoms of 512 B.  bf16 (X3):
-// LayoutType::SWIZZLE_64B (4), 8-pixel K atoms of 8 x 64 B = 512 B.  Either way SBO = 512 B and LBO = chunk distance.
-__device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t layout_type,
-                                                      uint32_t base_offset = 0) {
-    uint64_t d = static_cast<uint64_t>(base_offset & 7) << 49;   // swizzle-phase of a start address inside an atom
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;       // between 32-channel (MN) chunks
-    d |= static_cast<uint64_t>(512 >> 4) << 32;             // between K swizzle atoms
-    d |= static_cast<uint64_t>(1) << 46;                    // descriptor version (sm_100)
-    d |= static_cast<uint64_t>(layout_type) << 61;
-    return d;
-}
-
 constexpr int kHaloRows = kPix + 2;                 // 34 pixel rows: the 32 of the stage + one on each side
 
-// HALO (stride-1 layers with Ws >= 32): the KW shifted big-tensor tiles of a stage overlap in all but 2 pixel rows, so the
-// stage holds ONE (32 + 2)-row tile per 32-channel chunk and tap kw addresses it at row offset kw (start address + kw*128 B).
-// 35 KB instead of 64 KB per stage -> a 5-deep ring instead of 3 and 8 instead of 16 TMA issues.
+// HALO (fp32, stride-1 layers with Ws >= 32): the KW shifted big-tensor tiles of a stage overlap in all but 2 pixel rows, so
+// the stage holds ONE (32 + 2)-row tile per 32-channel chunk and tap kw reads it from pixel row kw on.
 template <int KW, int BLOCK_N, bool HALO = false, bool X3 = false>
 struct WgSmem {
     static constexpr int kRowBytes = X3 ? 64 : 128;                   // 32 channels of one pixel
     static constexpr int kChunkBytes = kPix * kRowBytes;              // one 32-channel x 32-pixel chunk: 4 KB fp32, 2 KB bf16
-    static constexpr int kHaloChunkBytes = X3 ? 2560 : 4608;          // 34 rows padded to a multiple of the 512 B swizzle atom
+    static constexpr int kHaloChunkBytes = 5120;                      // 34 rows of 128 B padded to the 1024 B swizzle atom
     static constexpr int kPlanes = X3 ? 2 : 1;                        // hi and lo chunk sets, hi first
     static constexpr int kBChunks = BLOCK_N / 32;
     static constexpr int kAPlaneBytes = kAChunks * kChunkBytes;
@@ -80,16 +67,21 @@ struct WgSmem {
     static constexpr int kTxBytes = HALO ? kABytes + kPlanes * kBChunks * kHaloRows * kRowBytes : kStageBytes;
     static constexpr int kBarrierOffset = (kStages * kStageBytes + 1023) / 1024 * 1024;
     static constexpr int kDynamic = kBarrierOffset + 128 + 1024;
-    static constexpr int kTmemCols = (KW * BLOCK_N <= 32) ? 32 : (KW * BLOCK_N <= 64) ? 64 : (KW * BLOCK_N <= 128) ? 128
-                                     : (KW * BLOCK_N <= 256) ? 256 : 512;
+    static_assert(!(HALO && X3), "the halo tile is an fp32-only layout");
 };
 
+// byte offset of (pixel row, channel) in a 32-channel fp32 chunk written by TMA with SWIZZLE_128B (1024 B aligned chunk):
+// the 16-byte column index is XOR-ed with the row index mod 8
+__device__ __forceinline__ uint32_t sw128_off(int row, int ch) {
+    return static_cast<uint32_t>(row * 128 + ((((ch >> 2) ^ row) & 7) << 4) + (ch & 3) * 4);
+}
+
 template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3>
-__global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_s,
-                                                          const __grid_constant__ CUtensorMap map_s2,
-                                                          const __grid_constant__ CUtensorMap map_b,
-                                                          const __grid_constant__ CUtensorMap map_b2,
-                                                          float* __restrict__ part, const WgParams p) {
+__global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_s,
+                                                                 const __grid_constant__ CUtensorMap map_s2,
+                                                                 const __grid_constant__ CUtensorMap map_b,
+                                                                 const __grid_constant__ CUtensorMap map_b2,
+                                                                 float* __restrict__ part, const WgParams p) {
     using L = WgSmem<KW, BLOCK_N, HALO, X3>;
     constexpr int kChunkBytes = L::kChunkBytes;
     constexpr int kHaloChunkBytes = L::kHaloChunkBytes;
@@ -98,8 +90,6 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarrierOffset);
     uint64_t* empty_bar = full_bar + kNStages;
-    uint64_t* tmem_full_bar = empty_bar + kNStages;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     const int ms = blockIdx.x;                       // 128-channel tile of the small tensor
@@ -110,35 +100,22 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
     const long long u1 = u0 + per < p.units ? u0 + per : p.units;
     const int iters = u1 > u0 ? static_cast<int>(u1 - u0) : 0;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kWgConsumerWarps && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_s) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         if (X3) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_s2) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b2) : "memory");
         }
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kNStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        mbar_init(tmem_full_bar, 1);
+        for (int s = 0; s < kNStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kWgConsumerWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(L::kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
-    if (iters > 0) {
-        if ((warp == 0 || (warp == 3 && !HALO)) && lane == 0) {
-            // ===================== TMA producers =====================
-            // Two issuing threads share the work of a stage (16 box loads of 4 KB): warp 0 arms the barrier and loads the
-            // S tile + the first Bg tap, warp 3 loads the remaining taps.  Both wait on the same empty barrier.
-            const bool first = warp == 0;
+    if (warp == kWgConsumerWarps) {
+        if (lane == 0) {
+            // ===================== TMA producer (one thread) =====================
             const int rows = kPix / p.pw;                    // rows of the small grid per stage
             const int segs = p.Ws / p.pw;                    // 32-pixel segments per row (>= 1 when pw == 32)
             const int row_bytes = p.pw * L::kRowBytes;
@@ -149,7 +126,7 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
                 mbar_wait(&empty_bar[stage], ph ^ 1);
                 uint8_t* a_dst = smem + stage * L::kStageBytes;
                 uint8_t* b_dst = a_dst + L::kABytes;
-                if (first) mbar_expect_tx(&full_bar[stage], L::kTxBytes);
+                mbar_expect_tx(&full_bar[stage], L::kTxBytes);
                 for (int r = 0; r < rows; ++r) {
                     long long grow;                          // global row index n*Hs + y
                     int x0;
@@ -161,7 +138,7 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
                         const CUtensorMap* ms_ = pl ? &map_s2 : &map_s;
                         const CUtensorMap* mb_ = pl ? &map_b2 : &map_b;
                         uint8_t* a_pl = a_dst + pl * L::kAPlaneBytes;
-                        if (first && (r == 0 || !p.mr_s)) {
+                        if (r == 0 || !p.mr_s) {
                             for (int c = 0; c < kAChunks; ++c) {
                                 if (STACK)   // chunk kh = S shifted by dy = 1 - kh rows (rows outside the image are zero-filled)
                                     tma_load_4d(a_pl + c * kChunkBytes + r * row_bytes, ms_, &full_bar[stage], 0, x0,
@@ -177,7 +154,7 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
                             continue;
                         }
                         if (r != 0 && p.mr_b) continue;
-                        for (int kw = first ? 0 : 1; kw < (first ? 1 : KW); ++kw)
+                        for (int kw = 0; kw < KW; ++kw)
                             for (int c = 0; c < L::kBChunks; ++c) {
                                 uint8_t* dst = b_dst + kw * L::kBBytesPerTap + pl * L::kBPlaneBytes + c * kChunkBytes + r * row_bytes;
                                 const int ch = nb * BLOCK_N + c * 32;
@@ -192,91 +169,139 @@ __global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const __grid_constant_
                 }
                 if (++stage == kNStages) { stage = 0; ph ^= 1; }
             }
-        } else if (warp == 1 && lane == 0) {
-            // ===================== MMA issuer =====================
-            // MN-major operands: a_major = b_major = 1 (bits 15, 16)
-            constexpr uint32_t idesc = (X3 ? make_idesc_bf16(128, BLOCK_N) : make_idesc_tf32(128, BLOCK_N)) | (1u << 15) | (1u << 16);
-            constexpr uint32_t kLayout = X3 ? 4u : 1u;       // SWIZZLE_64B (bf16) / SWIZZLE_128B_BASE32B (fp32)
-            constexpr uint32_t kBLbo = HALO ? kHaloChunkBytes : kChunkBytes;
-            int stage = 0;
-            uint32_t ph = 0;
-            for (int it = 0; it < iters; ++it) {
-                mbar_wait(&full_bar[stage], ph);
-                tcgen05_fence_after();
-                const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-                const uint64_t adesc = make_mnmajor_desc(a_addr, kChunkBytes, kLayout);
-                const uint64_t adesc_lo = make_mnmajor_desc(a_addr + L::kAPlaneBytes, kChunkBytes, kLayout);
+        }
+        return;
+    }
+
+    // ===================== consumers =====================
+    // The epilogue writes this split's slice of the partial buffer; a split without work (units not divisible) writes zeros,
+    // so the slice is always defined for the reduction.
+    float* pbase = part + split * p.part_stride;
+    const int g = lane >> 2, tq = lane & 3;
+    if (X3) {
+        // wgmma, both operands MN-major SWIZZLE_64B (rows of 64 B = 32 bf16, 8-pixel K atoms of 512 B): LBO = distance between
+        // 32-channel chunks, SBO = 512 B.  Warpgroup wg owns A chunks 2wg, 2wg+1 (its 64 rows); one accumulator per tap.
+        const int wg = warp >> 2, wq = warp & 3;
+        constexpr int kAcc = BLOCK_N / 2;
+        float acc[KW][kAcc];
+#pragma unroll
+        for (int kw = 0; kw < KW; ++kw)
+#pragma unroll
+            for (int i = 0; i < kAcc; ++i) acc[kw][i] = 0.f;
+        int stage = 0, prev = -1;
+        uint32_t ph = 0;
+        for (int it = 0; it < iters; ++it) {
+            mbar_wait(&full_bar[stage], ph);
+            const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
+            const uint64_t adesc = make_smem_desc(a_addr + wg * 2 * kChunkBytes, kChunkBytes, 512, 2);
+            const uint64_t adesc_lo = make_smem_desc(a_addr + L::kAPlaneBytes + wg * 2 * kChunkBytes, kChunkBytes, 512, 2);
+            wgmma_fence();
+#pragma unroll
+            for (int kw = 0; kw < KW; ++kw) {
+                fence_regs<kAcc>(acc[kw]);
+                const uint32_t b_addr = a_addr + L::kABytes + kw * L::kBBytesPerTap;
+                const uint64_t bdesc = make_smem_desc(b_addr, kChunkBytes, 512, 2);
+                const uint64_t bdesc_lo = make_smem_desc(b_addr + L::kBPlaneBytes, kChunkBytes, 512, 2);
+#pragma unroll
+                for (int j = 0; j < kPix / 16; ++j) {   // 16 pixels per MMA = two 8-pixel atoms: next slice = +1024 B (>>4 = 64)
+                    wgmma_bf16<BLOCK_N>(acc[kw], adesc_lo + 64 * j, bdesc + 64 * j, 1, Trans<1>());
+                    wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc_lo + 64 * j, 1, Trans<1>());
+                    wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc + 64 * j, 1, Trans<1>());
+                }
+            }
+            wgmma_commit();
+#pragma unroll
+            for (int kw = 0; kw < KW; ++kw) fence_regs<kAcc>(acc[kw]);
+            wgmma_wait<1>();
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == kNStages) { stage = 0; ph ^= 1; }
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int kw = 0; kw < KW; ++kw) fence_regs<kAcc>(acc[kw]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = wg * 64 + wq * 16 + g + 8 * h;      // row of the 128-row A tile
+            const int q = r >> 5;
+            if (STACK && q == 3) continue;                    // duplicate chunk
+            const int cs = STACK ? (r & 31) : ms * 128 + r;
+#pragma unroll
+            for (int kw = 0; kw < KW; ++kw) {
+                const int t = (STACK ? q : kh) * p.k + kw;
+                float* obase = pbase + (static_cast<long long>(t) * p.Cs + cs) * p.Cb + nb * BLOCK_N + 2 * tq;
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j)
+                    *reinterpret_cast<float2*>(obase + 8 * j) = make_float2(acc[kw][4 * j + 2 * h], acc[kw][4 * j + 2 * h + 1]);
+            }
+        }
+    } else {
+        // mma.sync m16n8k8 tf32: warp (wm, wn) computes rows 32wm..32wm+31 (= A chunk wm) x columns wn*BLOCK_N/2 .. of every
+        // tap.  Fragments are gathered from the SWIZZLE_128B tiles with 32-bit shared loads.
+        const int wm = warp & 3, wn = warp >> 2;
+        constexpr int NT = BLOCK_N / 16;                 // n8 tiles per warp
+        float acc[KW][2][NT][4];
+#pragma unroll
+        for (int kw = 0; kw < KW; ++kw)
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+                for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) acc[kw][mt][nt][e] = 0.f;
+        int stage = 0;
+        uint32_t ph = 0;
+        for (int it = 0; it < iters; ++it) {
+            mbar_wait(&full_bar[stage], ph);
+            const uint8_t* sa = smem + stage * L::kStageBytes + wm * kChunkBytes;
+            const uint8_t* sb = smem + stage * L::kStageBytes + L::kABytes;
+#pragma unroll
+            for (int k8 = 0; k8 < kPix / 8; ++k8) {
+                const int k0 = k8 * 8 + tq;
+                uint32_t a[2][4];
+#pragma unroll
+                for (int mt = 0; mt < 2; ++mt) {
+                    const int ch = mt * 16 + g;
+                    a[mt][0] = *reinterpret_cast<const uint32_t*>(sa + sw128_off(k0, ch));
+                    a[mt][1] = *reinterpret_cast<const uint32_t*>(sa + sw128_off(k0, ch + 8));
+                    a[mt][2] = *reinterpret_cast<const uint32_t*>(sa + sw128_off(k0 + 4, ch));
+                    a[mt][3] = *reinterpret_cast<const uint32_t*>(sa + sw128_off(k0 + 4, ch + 8));
+                }
 #pragma unroll
                 for (int kw = 0; kw < KW; ++kw) {
-                    // HALO: tap kw reads the one halo tile kw pixel rows further in
-                    const uint32_t b_addr = a_addr + L::kABytes + (HALO ? kw * L::kRowBytes : kw * L::kBBytesPerTap);
-                    const uint64_t bdesc = make_mnmajor_desc(b_addr, kBLbo, kLayout, (HALO && !X3 && p.halo_bo) ? kw : 0);
-                    if (X3) {
-                        const uint64_t bdesc_lo = make_mnmajor_desc(b_addr + L::kBPlaneBytes, kBLbo, kLayout);
 #pragma unroll
-                        for (int j = 0; j < kPix / 16; ++j) {   // 16 pixels per MMA = two 8-pixel atoms: next slice = +1024 B (>>4 = 64)
-                            umma_bf16(tmem_base + kw * BLOCK_N, adesc_lo + 64 * j, bdesc + 64 * j, idesc, (it | j) != 0);
-                            umma_bf16(tmem_base + kw * BLOCK_N, adesc + 64 * j, bdesc_lo + 64 * j, idesc, 1);
-                            umma_bf16(tmem_base + kw * BLOCK_N, adesc + 64 * j, bdesc + 64 * j, idesc, 1);
-                        }
-                    } else {
+                    for (int nt = 0; nt < NT; ++nt) {
+                        const int n = wn * (BLOCK_N / 2) + nt * 8 + g;
+                        const uint8_t* chunk = HALO ? sb + (n >> 5) * kHaloChunkBytes : sb + kw * L::kBBytesPerTap + (n >> 5) * kChunkBytes;
+                        const int row = HALO ? k0 + kw : k0;     // HALO: tap kw starts kw pixel rows into the halo tile
+                        uint32_t b[2];
+                        b[0] = *reinterpret_cast<const uint32_t*>(chunk + sw128_off(row, n & 31));
+                        b[1] = *reinterpret_cast<const uint32_t*>(chunk + sw128_off(row + 4, n & 31));
 #pragma unroll
-                        for (int j = 0; j < kPix / 8; ++j)   // 8 pixels per MMA: next swizzle atom = +1024 B (>>4 = 64)
-                            umma_tf32(tmem_base + kw * BLOCK_N, adesc + 64 * j, bdesc + 64 * j, idesc, (it | j) != 0);
+                        for (int mt = 0; mt < 2; ++mt) mma_tf32_m16n8k8(acc[kw][mt][nt], a[mt], b);
                     }
                 }
-                umma_commit(&empty_bar[stage]);
-                if (++stage == kNStages) { stage = 0; ph ^= 1; }
             }
-            umma_commit(tmem_full_bar);
-        } else if (warp >= 4) {
-            // ===================== epilogue: TMEM -> this split's slice of the partial buffer =====================
-            mbar_wait(tmem_full_bar, 0);
-            tcgen05_fence_after();
-            const int q = warp - 4;
-            const int cs = STACK ? lane : ms * 128 + q * 32 + lane;
-            float* pbase = part + split * p.part_stride;
-#pragma unroll 1
-            for (int kw = 0; kw < KW; ++kw) {
-                if (STACK && q == 3) break;                     // duplicate chunk
-                const int t = (STACK ? q : kh) * p.k + kw;
-                float* obase = pbase + (static_cast<long long>(t) * p.Cs + cs) * p.Cb + nb * BLOCK_N;
-#pragma unroll 1
-                for (int c = 0; c < BLOCK_N; c += 32) {
-                    uint32_t v[32];
-                    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + kw * BLOCK_N + c;
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                        : "r"(taddr));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            if (++stage == kNStages) { stage = 0; ph ^= 1; }
+        }
+        if (STACK && wm == 3) return;                           // duplicate chunk
 #pragma unroll
-                    for (int j = 0; j < 32; j += 8) st_global_v8(obase + c + j, v + j);
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = wm * 32 + mt * 16 + g + 8 * h;
+                const int cs = STACK ? (r & 31) : ms * 128 + r;
+#pragma unroll
+                for (int kw = 0; kw < KW; ++kw) {
+                    const int t = (STACK ? wm : kh) * p.k + kw;
+                    float* obase = pbase + (static_cast<long long>(t) * p.Cs + cs) * p.Cb + nb * BLOCK_N + wn * (BLOCK_N / 2) + 2 * tq;
+#pragma unroll
+                    for (int nt = 0; nt < NT; ++nt)
+                        *reinterpret_cast<float2*>(obase + nt * 8) = make_float2(acc[kw][mt][nt][2 * h], acc[kw][mt][nt][2 * h + 1]);
                 }
             }
-            tcgen05_fence_before();
-        }
-    } else if (warp >= 4) {
-        // a split without work (units not divisible): its slice must still be defined for the reduction
-        const int q = warp - 4;
-        const int cs = STACK ? lane : ms * 128 + q * 32 + lane;
-        float* pbase = part + split * p.part_stride;
-        for (int kw = 0; kw < KW; ++kw) {
-            if (STACK && q == 3) break;
-            const int t = (STACK ? q : kh) * p.k + kw;
-            float* obase = pbase + (static_cast<long long>(t) * p.Cs + cs) * p.Cb + nb * BLOCK_N;
-            for (int c = 0; c < BLOCK_N; c += 4) *reinterpret_cast<float4*>(obase + c) = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-    }
-    __syncthreads();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(L::kTmemCols) : "memory");
     }
 }
 
@@ -298,8 +323,8 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float* __restri
 
 inline bool pow2i(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
+// at most 64 big channels per CTA: KW accumulators of 128 x BLOCK_N live in the registers of the consumer warps
 int pick_bn(int Cb) {
-    if (Cb % 128 == 0) return 128;
     if (Cb % 64 == 0) return 64;
     if (Cb % 32 == 0) return 32;
     return 0;
@@ -317,7 +342,7 @@ int launch_wg(const WgMaps& m, float* out, float* part, const WgParams& p, cudaS
         attr_set = true;
     }
     dim3 grid(STACK ? 1 : p.Cs / 128, p.Cb / BLOCK_N, STACK ? p.splits : p.k * p.splits);
-    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3><<<grid, 256, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
+    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
     GIFB200_LAUNCH_CHECK("wgrad_tc_kernel");
     const int T = p.k * p.k;
     const long long total = static_cast<long long>(T) * p.Cs * p.Cb;
@@ -358,9 +383,8 @@ static long long wgrad_splits(int B, int Hi, int Wi, int Ci, int Ho, int Wo, int
     const int bn = pick_bn(Cb);
     const bool stack = (Cs == 32 && mode == 0 && k == 3);
     const long long base_ctas = stack ? (Cb / bn) : static_cast<long long>(Cs / 128) * (Cb / bn) * k;
-    // ONE wave: the kernel runs one CTA per SM (175-198 KB of shared memory), so the grid must not exceed the SM count.
-    // (Rounding the split count up gave 150 / 156 / 192 CTAs on 148 SMs: a second wave of 2-44 stragglers doubled the
-    // kernel time -- ncu run 33: tensor pipe busy 58% on the busiest SM but 30% on average.)
+    // ONE wave: the kernel runs one CTA per SM (130-160 KB of shared memory), so the grid must not exceed the SM count
+    // (rounding the split count up would leave a second wave of a few stragglers that doubles the kernel time).
     long long splits = kNumSMs / base_ctas;
     if (splits > units) splits = units;
     if (splits < 1) splits = 1;
@@ -376,11 +400,13 @@ size_t conv2d_wgrad_tc_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, in
 template <bool X3>
 static int dispatch_wg(int k, int bn, bool stack, bool halo, const WgMaps& m, float* gw, float* part, const WgParams& p, cudaStream_t st) {
 #define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3>(m, gw, part, p, st)
-    if (stack && halo) return bn == 128 ? GIFB200_WG(3, 128, true, true) : bn == 64 ? GIFB200_WG(3, 64, true, true) : GIFB200_WG(3, 32, true, true);
-    if (stack) return bn == 128 ? GIFB200_WG(3, 128, true, false) : bn == 64 ? GIFB200_WG(3, 64, true, false) : GIFB200_WG(3, 32, true, false);
-    if (halo) return bn == 128 ? GIFB200_WG(3, 128, false, true) : bn == 64 ? GIFB200_WG(3, 64, false, true) : GIFB200_WG(3, 32, false, true);
-    if (k == 3) return bn == 128 ? GIFB200_WG(3, 128, false, false) : bn == 64 ? GIFB200_WG(3, 64, false, false) : GIFB200_WG(3, 32, false, false);
-    return bn == 128 ? GIFB200_WG(1, 128, false, false) : bn == 64 ? GIFB200_WG(1, 64, false, false) : GIFB200_WG(1, 32, false, false);
+    if constexpr (!X3) {
+        if (stack && halo) return bn == 64 ? GIFB200_WG(3, 64, true, true) : GIFB200_WG(3, 32, true, true);
+        if (halo) return bn == 64 ? GIFB200_WG(3, 64, false, true) : GIFB200_WG(3, 32, false, true);
+    }
+    if (stack) return bn == 64 ? GIFB200_WG(3, 64, true, false) : GIFB200_WG(3, 32, true, false);
+    if (k == 3) return bn == 64 ? GIFB200_WG(3, 64, false, false) : GIFB200_WG(3, 32, false, false);
+    return bn == 64 ? GIFB200_WG(1, 64, false, false) : GIFB200_WG(1, 32, false, false);
 #undef GIFB200_WG
 }
 
@@ -411,9 +437,9 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
     const bool stack = (p.Cs == 32 && mode == 0 && k == 3);
     p.splits = static_cast<int>(wgrad_splits(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, nullptr));
     p.part_stride = static_cast<long long>(k) * k * Co * Ci;
-    // operand element size / tile layout: fp32 (MN-major SWIZZLE_128B_BASE32B) or bf16 planes (MN-major SWIZZLE_64B)
+    // operand element size / tile layout: fp32 (SWIZZLE_128B, read by mma.sync fragments) or bf16 planes (MN-major SWIZZLE_64B)
     const cuuint64_t es = x3 ? 2 : 4;
-    const CUtensorMapSwizzle swz = x3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B;
+    const CUtensorMapSwizzle swz = x3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
     const CUtensorMapDataType dt = x3 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
     const char* Sb = reinterpret_cast<const char*>(S);
     const char* Bb = reinterpret_cast<const char*>(Bg);
@@ -434,12 +460,10 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
         if (rc == GIFB200_OK && x3) rc = encode_map(&m.s2, Sb + s_plane, 4, dims, strides, box, swz, dt);
         if (rc != GIFB200_OK) return rc;
     }
-    // GIFB200_WGRAD_HALO: 0 = off, 1 = on (default).  Measured on B200: a tile start address that is a whole number of
-    // 128-byte rows into a swizzle atom needs base_offset = 0 (the swizzle is a function of the absolute shared-memory
-    // address bits); setting base_offset to the row phase (value 2 here) gives wrong results.
+    // GIFB200_WGRAD_HALO: 0 = off, 1 = on (default; fp32 operands only -- the bf16 planes are read by wgmma, which needs
+    // every tap tile to start on a swizzle atom).
     static const int halo_env = [] { const char* e = getenv("GIFB200_WGRAD_HALO"); return e ? atoi(e) : 1; }();
-    const bool halo = halo_env > 0 && mode == 0 && k == 3 && p.pw == kPix;
-    p.halo_bo = halo_env == 2;
+    const bool halo = halo_env > 0 && !x3 && mode == 0 && k == 3 && p.pw == kPix;
     if (!p.s2) {
         const cuuint64_t dims[4] = {static_cast<cuuint64_t>(p.Cb), static_cast<cuuint64_t>(p.Wb), static_cast<cuuint64_t>(p.Hb), static_cast<cuuint64_t>(B)};
         const cuuint64_t strides[3] = {static_cast<cuuint64_t>(p.Cb) * es, static_cast<cuuint64_t>(p.Wb) * p.Cb * es,

@@ -2,6 +2,8 @@
 // Roofline for all of them is HBM: algorithmic bytes = inputs read once + outputs written once.
 #include <cuda_bf16.h>
 
+#include <mutex>
+
 #include "common.cuh"
 
 namespace gifb200 {
@@ -85,8 +87,9 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------------ reductions
-// out[g,c] = sum_r x[g,r,c].  Block = 32 (channels) x 8 (row lanes); grid = (C/32, row chunks, G); partial sums
-// are combined with one atomicAdd per (block, channel) into the zero-initialised output.
+// out[g,c] = sum_r x[g,r,c].  Block = 32 (channels) x 8 (row lanes); grid = (C/32, row chunks, G).  The reductions below
+// store one partial sum per (row chunk, output element) in a Slots buffer (common.cuh): slot = blockIdx.y, G*C floats per
+// slot (the bias gradient of the tail kernels: slot = (b, row chunk), C floats per slot).
 __global__ void __launch_bounds__(256) rows_sum_kernel(const float* __restrict__ x, float* __restrict__ out, int rows,
                                                        int C, int rows_per_block) {
     __shared__ float sm[8][33];
@@ -105,7 +108,7 @@ __global__ void __launch_bounds__(256) rows_sum_kernel(const float* __restrict__
         float t = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
-        atomicAdd(out + static_cast<long long>(g) * C + c, t);
+        out[(static_cast<long long>(blockIdx.y) * gridDim.z + g) * C + c] = t;
     }
 }
 
@@ -131,7 +134,7 @@ __global__ void __launch_bounds__(256) spatial_dot_kernel(const float* __restric
         float t = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
-        atomicAdd(out + static_cast<long long>(g) * C + c, t);
+        out[(static_cast<long long>(blockIdx.y) * gridDim.z + g) * C + c] = t;
     }
 }
 
@@ -173,8 +176,8 @@ __global__ void __launch_bounds__(256) tail_bwd_kernel(const float* __restrict__
         float t = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) t += sm[threadIdx.y][j][threadIdx.x];
-        if (threadIdx.y == 0) { if (gb) atomicAdd(gb + c, t); }
-        else if (gd) atomicAdd(gd + static_cast<long long>(b) * C + c, t);
+        if (threadIdx.y == 0) { if (gb) gb[(static_cast<long long>(b) * gridDim.y + blockIdx.y) * C + c] = t; }
+        else if (gd) gd[(static_cast<long long>(blockIdx.y) * gridDim.z + b) * C + c] = t;
     }
 }
 
@@ -206,14 +209,14 @@ __global__ void __launch_bounds__(256) scale_bwd_kernel(const float* __restrict_
         float t = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
-        atomicAdd(gs + static_cast<long long>(b) * C + c, t);
+        gs[(static_cast<long long>(blockIdx.y) * gridDim.z + b) * C + c] = t;
     }
 }
 
 
 // 16-byte-per-lane variants of the two kernels above for C % 32 == 0 (every layer of the model): a thread owns 4
 // channels, TX lanes span TX*4 channels of one pixel row, 256/TX rows per block step; the row loop is unrolled so
-// that 8-12 independent 16-byte loads are in flight per thread (the scalar kernels reach ~2.7 TB/s, these ~HBM rate).
+// that 8-12 independent 16-byte loads are in flight per thread (a scalar kernel keeps too few bytes in flight to reach the HBM rate).
 // four consecutive elements of the two-term bf16 expansion (hi plane at planes[e], lo plane at planes[total + e])
 __device__ __forceinline__ void store_planes4(__nv_bfloat16* __restrict__ planes, long long total, long long e, const float4& t) {
     const __nv_bfloat16 h0 = __float2bfloat16_rn(t.x), h1 = __float2bfloat16_rn(t.y), h2 = __float2bfloat16_rn(t.z),
@@ -234,9 +237,7 @@ __device__ __forceinline__ void f4_add(float4& a, const float4& b) { a.x += b.x;
 __device__ __forceinline__ float4 f4_round(float4 v) {
     return make_float4(round_tf32(v.x), round_tf32(v.y), round_tf32(v.z), round_tf32(v.w));
 }
-__device__ __forceinline__ void f4_atomic_add(float* p, const float4& v) {
-    atomicAdd(p + 0, v.x); atomicAdd(p + 1, v.y); atomicAdd(p + 2, v.z); atomicAdd(p + 3, v.w);
-}
+__device__ __forceinline__ void f4_store(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
 
 template <int TX>
 __global__ void __launch_bounds__(256) tail_bwd_vec_kernel(const float* __restrict__ gy, const float* __restrict__ y,
@@ -283,8 +284,8 @@ __global__ void __launch_bounds__(256) tail_bwd_vec_kernel(const float* __restri
         float4 t = f4_zero();
 #pragma unroll
         for (int j = 0; j < TY; ++j) f4_add(t, sm[ty][j][tx]);
-        if (ty == 0) { if (gb) f4_atomic_add(gb + c, t); }
-        else if (gd) f4_atomic_add(gd + static_cast<long long>(b) * C + c, t);
+        if (ty == 0) { if (gb) f4_store(gb + (static_cast<long long>(b) * gridDim.y + blockIdx.y) * C + c, t); }
+        else if (gd) f4_store(gd + (static_cast<long long>(blockIdx.y) * gridDim.z + b) * C + c, t);
     }
 }
 
@@ -319,7 +320,7 @@ __global__ void __launch_bounds__(256) scale_bwd_vec_kernel(const float* __restr
         float4 t = f4_zero();
 #pragma unroll
         for (int j = 0; j < TY; ++j) f4_add(t, sm[j][tx]);
-        f4_atomic_add(gs + static_cast<long long>(b) * C + c, t);
+        f4_store(gs + (static_cast<long long>(blockIdx.y) * gridDim.z + b) * C + c, t);
     }
 }
 
@@ -362,7 +363,7 @@ __global__ void __launch_bounds__(256) tail_bwd2_kernel(const float* __restrict_
         float t = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
-        atomicAdd(gdd + static_cast<long long>(b) * C + c, t);
+        gdd[(static_cast<long long>(blockIdx.y) * gridDim.z + b) * C + c] = t;
     }
 }
 
@@ -417,7 +418,7 @@ __global__ void __launch_bounds__(256) tail_bwd2_vec_kernel(const float* __restr
         float4 t = f4_zero();
 #pragma unroll
         for (int j = 0; j < TY; ++j) f4_add(t, sm[j][tx]);
-        f4_atomic_add(gdd + static_cast<long long>(b) * C + c, t);
+        f4_store(gdd + (static_cast<long long>(blockIdx.y) * gridDim.z + b) * C + c, t);
     }
 }
 
@@ -578,7 +579,7 @@ __global__ void __launch_bounds__(256) torgb_bwd_x_kernel(const float* __restric
     }
 }
 
-// gws[b,k,i] = sum_p gy[b,p,k]*x[b,p,i]   (block: 32 channels x 8 row lanes, atomics into zeroed output)
+// gws[b,k,i] = sum_p gy[b,p,k]*x[b,p,i]   (block: 32 channels x 8 row lanes, partial sums into slots)
 __global__ void __launch_bounds__(256) torgb_bwd_w_kernel(const float* __restrict__ gy, const float* __restrict__ x,
                                                           float* __restrict__ gws, int P, int C, int rows_per_block) {
     __shared__ float sm[3][8][33];
@@ -603,14 +604,14 @@ __global__ void __launch_bounds__(256) torgb_bwd_w_kernel(const float* __restric
         float t = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) t += sm[threadIdx.y][j][threadIdx.x];
-        atomicAdd(gws + (static_cast<long long>(b) * 3 + threadIdx.y) * C + c, t);
+        gws[((static_cast<long long>(blockIdx.y) * gridDim.z + b) * 3 + threadIdx.y) * C + c] = t;
     }
 }
 
 
 // 16-byte variants of the three ToRGB kernels for C % 32 == 0 (same lane layout as tail_bwd_vec_kernel: a thread owns 4
 // channels, TX lanes span a pixel's channel chunk, 256/TX pixels per block step, rows unrolled for loads in flight).
-// The scalar versions sat at 2.3 TB/s (one 16-byte load in flight per lane and 15 shuffles per pixel in the forward).
+// The scalar versions kept one 16-byte load in flight per lane and spent 15 shuffles per pixel in the forward.
 template <int TX>
 __global__ void __launch_bounds__(256) torgb_fwd_vec_kernel(const float* __restrict__ x, const float* __restrict__ ws,
                                                             float* __restrict__ y, int P, int C, int rows_per_block) {
@@ -705,7 +706,7 @@ __global__ void __launch_bounds__(256) torgb_bwd_w_vec_kernel(const float* __res
         float4 t = f4_zero();
 #pragma unroll
         for (int j = 0; j < TY; ++j) f4_add(t, sm[ty][j][tx]);
-        f4_atomic_add(gws + (static_cast<long long>(b) * 3 + ty) * C + c, t);
+        f4_store(gws + ((static_cast<long long>(blockIdx.y) * gridDim.z + b) * 3 + ty) * C + c, t);
     }
 }
 
@@ -757,6 +758,51 @@ static inline int grid_for(long long work_items, int per_block) {
 }  // namespace gifb200
 
 using namespace gifb200;
+
+namespace gifb200 {
+
+__global__ void __launch_bounds__(256) slots_reduce_kernel(const float* __restrict__ part, float* __restrict__ out, int slots,
+                                                           long long n) {
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        float t = 0.f;
+        for (int k = 0; k < slots; ++k) t += part[k * n + i];
+        out[i] = t;
+    }
+}
+
+int slots_take(Slots& s, float*& out, int count, long long n, cudaStream_t st) {
+    // keep freed slot buffers in the stream-ordered pool instead of returning them to the driver at every synchronisation
+    static std::once_flag keep;
+    std::call_once(keep, [] {
+        int dev = 0;
+        cudaMemPool_t pool;
+        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+            uint64_t keep_all = UINT64_MAX;
+            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep_all);
+        }
+    });
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&s.part), sizeof(float) * static_cast<size_t>(count) * n, st);
+    if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "partial-sum buffer", cudaGetErrorString(e));
+    s.out = out;
+    s.count = count;
+    s.n = n;
+    out = s.part;
+    return GIFB200_OK;
+}
+
+int slots_reduce(Slots& s, cudaStream_t st) {
+    int blocks = cdiv(s.n, 256);
+    if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+    slots_reduce_kernel<<<blocks, 256, 0, st>>>(s.part, s.out, s.count, s.n);
+    const int rc = check_launch("slots_reduce_kernel");
+    cudaError_t e = cudaFreeAsync(s.part, st);
+    s.part = nullptr;
+    if (rc != GIFB200_OK) return rc;
+    return e == cudaSuccess ? GIFB200_OK : fail(GIFB200_E_CUDA, "partial-sum buffer", cudaGetErrorString(e));
+}
+
+}  // namespace gifb200
 
 extern "C" {
 
@@ -828,9 +874,11 @@ int gifb200_rows_sum(const float* x, float* out, int G, int rows, int C, gifb200
     int rpb;
     const int rb = rows_split(rows, cb, G, &rpb);
     GIFB200_REQUIRE(G <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "rows_sum: grid too large");
+    Slots sl;
+    if (int rc = slots_take(sl, out, rb, static_cast<long long>(G) * C, st)) return rc;
     rows_sum_kernel<<<dim3(cb, rb, G), dim3(32, 8), 0, st>>>(x, out, rows, C, rpb);
     GIFB200_LAUNCH_CHECK("rows_sum_kernel");
-    return GIFB200_OK;
+    return slots_reduce(sl, st);
 }
 
 int gifb200_spatial_dot(const float* a, const float* b2, float* out, int B, int P, int C, gifb200_stream_t stream) {
@@ -844,9 +892,22 @@ int gifb200_spatial_dot(const float* a, const float* b2, float* out, int B, int 
     int rpb;
     const int rb = rows_split(P, cb, B, &rpb);
     GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "spatial_dot: grid too large");
+    Slots sl;
+    if (int rc = slots_take(sl, out, rb, static_cast<long long>(B) * C, st)) return rc;
     spatial_dot_kernel<<<dim3(cb, rb, B), dim3(32, 8), 0, st>>>(a, b2, out, P, C, rpb);
     GIFB200_LAUNCH_CHECK("spatial_dot_kernel");
-    return GIFB200_OK;
+    return slots_reduce(sl, st);
+}
+
+// gb: one slot per (b, row chunk); gd: one per row chunk (either may be absent)
+static int tail_slots(Slots& sb, Slots& sd, float*& gb, float*& gd, int B, int rb, int C, cudaStream_t st) {
+    int rc = gb ? slots_take(sb, gb, B * rb, C, st) : GIFB200_OK;
+    return rc == GIFB200_OK && gd ? slots_take(sd, gd, rb, static_cast<long long>(B) * C, st) : rc;
+}
+
+static int tail_reduce(Slots& sb, Slots& sd, cudaStream_t st) {
+    int rc = sb.part ? slots_reduce(sb, st) : GIFB200_OK;
+    return rc == GIFB200_OK && sd.part ? slots_reduce(sd, st) : rc;
 }
 
 static int tail_bwd_impl(const float* gy, const float* y, const float* acc, const float* d, float* gt, float* gacc,
@@ -874,6 +935,8 @@ static int tail_bwd_impl(const float* gy, const float* y, const float* acc, cons
         const int rb = rows_split_vec(P, cbv, B, 256 / tx, &rpb);
         GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "tail_bwd: grid too large");
         const dim3 grid(cbv, rb, B);
+        Slots sb, sd;
+        if (int rc = tail_slots(sb, sd, gb, gd, B, rb, C, st)) return rc;
         __nv_bfloat16* p1 = static_cast<__nv_bfloat16*>(gt_planes);
         __nv_bfloat16* p2 = static_cast<__nv_bfloat16*>(gacc_planes);
         const long long total = static_cast<long long>(B) * P * C;
@@ -881,16 +944,18 @@ static int tail_bwd_impl(const float* gy, const float* y, const float* acc, cons
         else if (tx == 16) tail_bwd_vec_kernel<16><<<grid, 256, 0, st>>>(gy, y, acc, d, gt, gacc, gb, gd, P, C, rpb, slope, gain, rtf32, p1, p2, total);
         else tail_bwd_vec_kernel<8><<<grid, 256, 0, st>>>(gy, y, acc, d, gt, gacc, gb, gd, P, C, rpb, slope, gain, rtf32, p1, p2, total);
         GIFB200_LAUNCH_CHECK("tail_bwd_vec_kernel");
-        return GIFB200_OK;
+        return tail_reduce(sb, sd, st);
     }
     GIFB200_REQUIRE(!planes, GIFB200_E_ALIGN, "tail_bwd: the planes outputs need C % 32 == 0 and 16-byte aligned pointers");
     const int cb = cdiv(C, 32);
     int rpb;
     const int rb = rows_split(P, cb, B, &rpb);
     GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "tail_bwd: grid too large");
+    Slots sb, sd;
+    if (int rc = tail_slots(sb, sd, gb, gd, B, rb, C, st)) return rc;
     tail_bwd_kernel<<<dim3(cb, rb, B), dim3(32, 8), 0, st>>>(gy, y, acc, d, gt, gacc, gb, gd, P, C, rpb, slope, gain, rtf32);
     GIFB200_LAUNCH_CHECK("tail_bwd_kernel");
-    return GIFB200_OK;
+    return tail_reduce(sb, sd, st);
 }
 
 int gifb200_tail_bwd(const float* gy, const float* y, const float* acc, const float* d, float* gt, float* gacc,
@@ -919,19 +984,23 @@ int gifb200_scale_bwd(const float* gy, const float* x, const float* s, float* gx
         const int rb = rows_split_vec(P, cbv, B, 256 / tx, &rpb);
         GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "scale_bwd: grid too large");
         const dim3 grid(cbv, rb, B);
+        Slots sl;
+        if (int rc = slots_take(sl, gs, rb, static_cast<long long>(B) * C, st)) return rc;
         if (tx == 32) scale_bwd_vec_kernel<32><<<grid, 256, 0, st>>>(gy, x, s, gx, gs, P, C, rpb, rtf32);
         else if (tx == 16) scale_bwd_vec_kernel<16><<<grid, 256, 0, st>>>(gy, x, s, gx, gs, P, C, rpb, rtf32);
         else scale_bwd_vec_kernel<8><<<grid, 256, 0, st>>>(gy, x, s, gx, gs, P, C, rpb, rtf32);
         GIFB200_LAUNCH_CHECK("scale_bwd_vec_kernel");
-        return GIFB200_OK;
+        return slots_reduce(sl, st);
     }
     const int cb = cdiv(C, 32);
     int rpb;
     const int rb = rows_split(P, cb, B, &rpb);
     GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "scale_bwd: grid too large");
+    Slots sl;
+    if (int rc = slots_take(sl, gs, rb, static_cast<long long>(B) * C, st)) return rc;
     scale_bwd_kernel<<<dim3(cb, rb, B), dim3(32, 8), 0, st>>>(gy, x, s, gx, gs, P, C, rpb, rtf32);
     GIFB200_LAUNCH_CHECK("scale_bwd_kernel");
-    return GIFB200_OK;
+    return slots_reduce(sl, st);
 }
 
 int gifb200_tail_bwd2(const float* gg, const float* ggd, const float* gy, const float* y, const float* acc, const float* d,
@@ -956,22 +1025,26 @@ int gifb200_tail_bwd2(const float* gg, const float* ggd, const float* gy, const 
         const int rb = rows_split_vec(P, cbv, B, 256 / tx, &rpb);
         GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "tail_bwd2: grid too large");
         const dim3 grid(cbv, rb, B);
+        Slots sl;
+        if (int rc = gdd && gg ? slots_take(sl, gdd, rb, static_cast<long long>(B) * C, st) : GIFB200_OK) return rc;
         __nv_bfloat16* pp = static_cast<__nv_bfloat16*>(ggy_planes);
         const long long total = static_cast<long long>(B) * P * C;
         if (tx == 32) tail_bwd2_vec_kernel<32><<<grid, 256, 0, st>>>(gg, ggd, gy, y, acc, d, ggy, gx2, gdd, P, C, rpb, slope, gain, pp, total);
         else if (tx == 16) tail_bwd2_vec_kernel<16><<<grid, 256, 0, st>>>(gg, ggd, gy, y, acc, d, ggy, gx2, gdd, P, C, rpb, slope, gain, pp, total);
         else tail_bwd2_vec_kernel<8><<<grid, 256, 0, st>>>(gg, ggd, gy, y, acc, d, ggy, gx2, gdd, P, C, rpb, slope, gain, pp, total);
         GIFB200_LAUNCH_CHECK("tail_bwd2_vec_kernel");
-        return GIFB200_OK;
+        return sl.part ? slots_reduce(sl, st) : GIFB200_OK;
     }
     GIFB200_REQUIRE(!ggy_planes, GIFB200_E_ALIGN, "tail_bwd2: the planes output needs C % 32 == 0 and 16-byte aligned pointers");
     const int cb = cdiv(C, 32);
     int rpb;
     const int rb = rows_split(P, cb, B, &rpb);
     GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "tail_bwd2: grid too large");
+    Slots sl;
+    if (int rc = gdd && gg ? slots_take(sl, gdd, rb, static_cast<long long>(B) * C, st) : GIFB200_OK) return rc;
     tail_bwd2_kernel<<<dim3(cb, rb, B), dim3(32, 8), 0, st>>>(gg, ggd, gy, y, acc, d, ggy, gx2, gdd, P, C, rpb, slope, gain);
     GIFB200_LAUNCH_CHECK("tail_bwd2_kernel");
-    return GIFB200_OK;
+    return sl.part ? slots_reduce(sl, st) : GIFB200_OK;
 }
 
 int gifb200_chan_scale(const float* x, const float* s, float* y, int B, int P, int C, int rtf32,
@@ -1080,19 +1153,23 @@ int gifb200_torgb_bwd_w(const float* gy, const float* x, float* gws, int B, int 
         const int rbv = rows_split_vec(P, cbv, B, 256 / tx, &rpbv);
         GIFB200_REQUIRE(B <= 65535 && rbv <= 65535, GIFB200_E_SHAPE, "torgb_bwd_w: grid too large");
         const dim3 grid(cbv, rbv, B);
+        Slots sl;
+        if (int rc = slots_take(sl, gws, rbv, static_cast<long long>(B) * 3 * C, st)) return rc;
         if (tx == 32) torgb_bwd_w_vec_kernel<32><<<grid, 256, 0, st>>>(gy, x, gws, P, C, rpbv);
         else if (tx == 16) torgb_bwd_w_vec_kernel<16><<<grid, 256, 0, st>>>(gy, x, gws, P, C, rpbv);
         else torgb_bwd_w_vec_kernel<8><<<grid, 256, 0, st>>>(gy, x, gws, P, C, rpbv);
         GIFB200_LAUNCH_CHECK("torgb_bwd_w_vec_kernel");
-        return GIFB200_OK;
+        return slots_reduce(sl, st);
     }
     const int cb = cdiv(C, 32);
     int rpb;
     const int rb = rows_split(P, cb, B, &rpb);
     GIFB200_REQUIRE(B <= 65535 && rb <= 65535, GIFB200_E_SHAPE, "torgb_bwd_w: grid too large");
+    Slots sl;
+    if (int rc = slots_take(sl, gws, rb, static_cast<long long>(B) * 3 * C, st)) return rc;
     torgb_bwd_w_kernel<<<dim3(cb, rb, B), dim3(32, 8), 0, st>>>(gy, x, gws, P, C, rpb);
     GIFB200_LAUNCH_CHECK("torgb_bwd_w_kernel");
-    return GIFB200_OK;
+    return slots_reduce(sl, st);
 }
 
 int gifb200_cond_down(float* x, float* y, int B, int H, int W, int C, int s, int adjoint, gifb200_stream_t stream) {

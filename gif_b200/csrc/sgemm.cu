@@ -1,6 +1,6 @@
 // Small dense fp32 GEMM for EqualLinear (mapping network 512x512, modulation 512xCi, D head 8192x512):
 // C[M,N] = alpha * op(A) op(B).  32x32 tiles, 256 threads, 2x2 micro-tiles.  These GEMMs are tiny
-// (<= 0.3 GFLOP per step in total) so a SIMT kernel is the right tool; tcgen05 is reserved for the convolutions.
+// (<= 0.3 GFLOP per step in total) so a SIMT kernel is the right tool; the tensor cores are reserved for the convolutions.
 #include "common.cuh"
 
 namespace gifb200 {
@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(int transA, int transB, int 
             const int gm = m0 + ty * 2 + i, gn = n0 + tx * 2 + j;
             if (gm < M && gn < N) {
                 if (gridDim.z == 1) C[static_cast<long long>(gm) * ldc + gn] = alpha * acc[i][j];
-                else atomicAdd(C + static_cast<long long>(gm) * ldc + gn, alpha * acc[i][j]);   // split-K into zeroed C
+                else C[(static_cast<long long>(blockIdx.z) * M + gm) * N + gn] = alpha * acc[i][j];   // split-K: C = slots
             }
         }
 }
@@ -65,8 +65,8 @@ extern "C" int gifb200_sgemm(int transA, int transB, int M, int N, int K, float 
     // few output tiles and a long K (the 8192 -> 512 discriminator head, its gradients): split K across CTAs
     const long long tiles = static_cast<long long>(cdiv(N, 32)) * cdiv(M, 32);
     int splits = 1;
-    // ... and the batch-32 style / mapping-network GEMMs (M = 32, N = K = 512: 16 output tiles, 16 serial k-tiles each was
-    // 27 us of latency per launch, 250 launches per step): at least two k-tiles per split
+    // ... and the batch-32 style / mapping-network GEMMs (M = 32, N = K = 512: 16 output tiles of 16 serial k-tiles each are
+    // latency-bound, 250 launches per step): at least two k-tiles per split
     if (tiles < kNumSMs && K >= 128 && ldc == N) {
         splits = static_cast<int>((2LL * kNumSMs + tiles - 1) / tiles);
         const int max_splits = K >= 1024 ? K / 256 : K / 64;
@@ -75,13 +75,13 @@ extern "C" int gifb200_sgemm(int transA, int transB, int M, int N, int K, float 
     }
     int kps = ((K + splits - 1) / splits + 31) / 32 * 32;
     splits = (K + kps - 1) / kps;
+    Slots sl;      // split-K: one partial product per split, added in split order
     if (splits > 1) {
         GIFB200_REQUIRE(ldc == N, GIFB200_E_SHAPE, "sgemm: split-K needs a dense C");
-        cudaError_t e = cudaMemsetAsync(C, 0, sizeof(float) * static_cast<size_t>(M) * N, st);
-        if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "sgemm memset", cudaGetErrorString(e));
+        if (int rc = slots_take(sl, C, splits, static_cast<long long>(M) * N, st)) return rc;
     }
     sgemm_kernel<<<dim3(cdiv(N, 32), cdiv(M, 32), splits), 256, 0, st>>>(transA, transB, M, N, K, alpha, A, lda, B, ldb, C,
                                                                          ldc, kps);
     GIFB200_LAUNCH_CHECK("sgemm_kernel");
-    return GIFB200_OK;
+    return sl.part ? slots_reduce(sl, st) : GIFB200_OK;
 }

@@ -1,4 +1,4 @@
-// Shared tcgen05 / TMA / mbarrier plumbing for the sm_100a tensor-core kernels (conv_tc.cu, conv_wgrad_tc.cu).
+// Shared wgmma / TMA / mbarrier plumbing for the sm_90a tensor-core kernels (conv_tc.cu, conv_wgrad_tc.cu).
 #pragma once
 #include <cuda.h>
 
@@ -17,6 +17,10 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
         "{\n"
@@ -50,72 +54,89 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* map, u
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
-// one 256-bit store (STG.E.256): 8 consecutive fp32 (as raw bits) to a 32-byte aligned address
-__device__ __forceinline__ void st_global_v8(float* dst, const uint32_t* v) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-                 "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
+// ----------------------------------------------------------------------------------------------- wgmma (sm_90a)
+// Warpgroup MMA: D (registers of the 128 threads of a warpgroup, m64nN fp32) (+)= A[smem desc] * B[smem desc].
+// Accumulator fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[4j + 2h + e] is row 16w + l/4 + 8h,
+// column 8j + 2(l%4) + e.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float* d) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16 operands, fp32 accumulate): the products of the bf16x3
-// error-compensated contraction
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major, SWIZZLE_64B descriptor (rows of 64 bytes = 32 bf16; SBO = 8 rows x 64 B = 512 B; layout_type 4)
-__device__ __forceinline__ uint64_t make_kmajor_sw64_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>(1) << 16;
-    d |= static_cast<uint64_t>(512 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(4) << 61;
-    return d;
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp):
-// start>>4 [0,14) | LBO>>4 [16,30) (=1, unused for swizzled K-major) | SBO>>4 [32,46) (=1024 B: 8 rows x 128 B) |
-// version=1 [46,48) | layout_type=SWIZZLE_128B(2) [61,64)
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>(1) << 16;
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-// cute::UMMA::InstrDescriptor: c_format F32 (1) [4,6) | a_format TF32 (2) [7,10) | b_format TF32 (2) [10,13) |
-// a_major K (0) [15] | b_major K (0) [16] | N>>3 [17,23) | M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+template <int V>
+struct Trans {};
+// kind tf32: both operands K-major (the only layout wgmma accepts for 32-bit types); K = 8 per instruction
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, int scale_d);
+// bf16 operands, fp32 accumulate, K = 16 per instruction; Trans<1>: both operands MN-major (transposed)
+template <int N, int T>
+__device__ __forceinline__ void wgmma_bf16(float* d, uint64_t da, uint64_t db, int scale_d, Trans<T>);
+// operand lists of the accumulator fragment: N/2 "+f" registers, and the matching "%0, %1, ..." of the PTX template
+#define GIF_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define GIF_F16 GIF_F8(0), GIF_F8(8)
+#define GIF_F32 GIF_F16, GIF_F8(16), GIF_F8(24)
+#define GIF_F64 GIF_F32, GIF_F8(32), GIF_F8(40), GIF_F8(48), GIF_F8(56)
+#define GIF_R8(a, b, c, d, e, f, g, h) "%" #a ", %" #b ", %" #c ", %" #d ", %" #e ", %" #f ", %" #g ", %" #h
+#define GIF_R16 GIF_R8(0, 1, 2, 3, 4, 5, 6, 7) ", " GIF_R8(8, 9, 10, 11, 12, 13, 14, 15)
+#define GIF_R32 GIF_R16 ", " GIF_R8(16, 17, 18, 19, 20, 21, 22, 23) ", " GIF_R8(24, 25, 26, 27, 28, 29, 30, 31)
+#define GIF_R64 GIF_R32 ", " GIF_R8(32, 33, 34, 35, 36, 37, 38, 39) ", " GIF_R8(40, 41, 42, 43, 44, 45, 46, 47) ", " \
+    GIF_R8(48, 49, 50, 51, 52, 53, 54, 55) ", " GIF_R8(56, 57, 58, 59, 60, 61, 62, 63)
+// operands after the accumulators: descriptors %R, %R+1, scale-d %R+2 (, transpose immediates %R+3, %R+4)
+#define GIF_WGMMA_TF32(N, R, S0, S1, S2) \
+    template <> \
+    __device__ __forceinline__ void wgmma_tf32<N>(float* d, uint64_t da, uint64_t db, int scale_d) { \
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #S2 ", 0;\n" \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k8.f32.tf32.tf32 {" GIF_R##R "}, %" #S0 ", %" #S1 \
+                     ", p, 1, 1;\n}\n" \
+                     : GIF_F##R \
+                     : "l"(da), "l"(db), "r"(scale_d)); \
+    }
+#define GIF_WGMMA_BF16(N, R, S0, S1, S2, T0, T1, TR) \
+    template <> \
+    __device__ __forceinline__ void wgmma_bf16<N>(float* d, uint64_t da, uint64_t db, int scale_d, Trans<TR>) { \
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #S2 ", 0;\n" \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" GIF_R##R "}, %" #S0 ", %" #S1 \
+                     ", p, 1, 1, %" #T0 ", %" #T1 ";\n}\n" \
+                     : GIF_F##R \
+                     : "l"(da), "l"(db), "r"(scale_d), "n"(TR), "n"(TR)); \
+    }
+GIF_WGMMA_TF32(32, 16, 16, 17, 18)
+GIF_WGMMA_TF32(64, 32, 32, 33, 34)
+GIF_WGMMA_TF32(128, 64, 64, 65, 66)
+GIF_WGMMA_BF16(32, 16, 16, 17, 18, 19, 20, 0)
+GIF_WGMMA_BF16(64, 32, 32, 33, 34, 35, 36, 0)
+GIF_WGMMA_BF16(128, 64, 64, 65, 66, 67, 68, 0)
+GIF_WGMMA_BF16(32, 16, 16, 17, 18, 19, 20, 1)
+GIF_WGMMA_BF16(64, 32, 32, 33, 34, 35, 36, 1)
+
+// warp-level tensor-core MMA, m16n8k8, tf32 operands, fp32 accumulate (the weight-gradient kernel's tf32 mode: its operands
+// are MN-major in shared memory, which wgmma does not accept for 32-bit types, so the fragments are gathered with lds)
+__device__ __forceinline__ void mma_tf32_m16n8k8(float* c, const uint32_t* a, const uint32_t* b) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-// same with a_format = b_format = BF16 (1) for kind::f16
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+// Shared-memory matrix descriptor (sm_90 GMMA): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | base_offset [49,52) |
+// layout [62,64): 1 = SWIZZLE_128B, 2 = SWIZZLE_64B
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
+    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
+    d |= static_cast<uint64_t>(layout) << 62;
+    return d;
 }
+// K-major, SWIZZLE_128B (rows of 128 bytes = 32 fp32; 8-row atoms of 1024 B)
+__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) { return make_smem_desc(smem_addr, 16, 1024, 1); }
+// K-major, SWIZZLE_64B (rows of 64 bytes = 32 bf16; 8-row atoms of 512 B)
+__device__ __forceinline__ uint64_t make_kmajor_sw64_desc(uint32_t smem_addr) { return make_smem_desc(smem_addr, 16, 512, 2); }
 
 // ----------------------------------------------------------------------------------------------- host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

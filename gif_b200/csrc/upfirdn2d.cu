@@ -127,9 +127,8 @@ constexpr int kDT = 8;                  // output tile edge
 constexpr int kDTI = 2 * kDT + 2;       // input tile edge
 // ------------------------------------------------------------------------------------------------ pipelined 4x4 FIR
 // Persistent, double-buffered shared-memory FIR (C % 32 == 0, 4x4 kernel, up = 1, down = 1 or 2).
-// ncu on the single-buffered blur (profiles/r01_ncu_upfirdn_blur.md): DRAM traffic is already algorithmic (1.07 GB in,
-// 1.04 GB out) but the kernel sits at 3.0 TB/s with `long_scoreboard` as the top stall -- a CTA loads its tile, waits,
-// computes, and 4 CTAs per SM (register + smem limit) do not keep enough bytes in flight.  Here a CTA walks a list of
+// A single-buffered blur moves only the algorithmic DRAM bytes but stalls on `long_scoreboard` -- a CTA loads its tile,
+// waits, computes, and 4 CTAs per SM (register + smem limit) do not keep enough bytes in flight.  Here a CTA walks a list of
 // tiles and issues the cp.async (LDGSTS, zero-fill for the padding) loads of tile i+1 before it computes tile i, so
 // every SM always has 2 x 41-46 KB of reads in flight underneath the FMAs and stores.
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, int src_bytes) {

@@ -111,7 +111,7 @@ def _conv_mode(kernel_size, stride, padding):
 
 def _pad_channels_for_tc(x, wt):
     """tensor-core modes (tf32 / bf16x3): zero-pad the input channels (and the weight's Ci) to a multiple of 32 so that odd-channel layers (the
-    9-channel discriminator stem, the 513-channel minibatch-stddev conv) run on the tcgen05 kernels; values unchanged."""
+    9-channel discriminator stem, the 513-channel minibatch-stddev conv) run on the tensor-core kernels; values unchanged."""
     ci = x.shape[-1]
     if ops.tc_enabled() and ci % 32 != 0 and wt.shape[1] % 32 == 0:
         pad = 32 - ci % 32
@@ -279,7 +279,7 @@ class NoiseInjection(nn.Module):
         """noise (B,r,r,c) NHWC -> (B,r,r,Co) NHWC *without* the last bias (returned separately for fusion).
 
         In tf32 mode the 6/12/24-channel tensors are zero-padded to 32 channels (weights and biases padded to match, so
-        the values are unchanged) which makes all three convolutions eligible for the tcgen05 kernel: 5x more nominal
+        the values are unchanged) which makes all three convolutions eligible for the tensor-core kernel: 5x more nominal
         FLOPs on the first one, but on a pipe that is ~50x faster than the fp32 SIMT path."""
         c0, c2, c4 = self.noise_conv[0], self.noise_conv[2], self.noise_conv[4]
         w0, w2, w4 = ops.prep_weight(c0.weight), ops.prep_weight(c2.weight), ops.prep_weight(c4.weight)

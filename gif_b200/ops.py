@@ -19,7 +19,7 @@ from ._lib import check, lib, ptr, require_cuda, stream
 
 S1, S2, T2 = 0, 1, 2          # conv modes of gifb200_conv2d
 _ADJ_MODE = {S1: S1, S2: T2, T2: S2}
-CONV_IMPL = 0                 # 0 auto, 1 force SIMT fp32, 2 force tcgen05 (tests flip this)
+CONV_IMPL = 0                 # 0 auto, 1 force SIMT fp32, 2 force the tensor-core path (tests flip this)
 WGRAD_IMPL = 0                # same for the weight-gradient kernel
 _PRECISION = "tf32"
 
@@ -47,10 +47,10 @@ class input_gradient_only:
 
 
 def set_precision(mode):
-    """"tf32":   convolutions that qualify run on tcgen05 (kind::tf32, fp32 accumulate) and their operand producers round
+    """"tf32":   convolutions that qualify run on the tensor cores (tf32, fp32 accumulate) and their operand producers round
                  to tf32 (~3e-4 per operator);
     "bf16x3": the same kernels in their error-compensated mode -- operands split into two bf16 terms
-                 (gifb200_split_bf16), three kind::f16 MMAs per slice, fp32 accumulate: ~1e-5 per operator at 1.5x the
+                 (gifb200_split_bf16), three bf16 MMAs per slice, fp32 accumulate: ~1e-5 per operator at 1.5x the
                  tensor work; the mode that holds BASELINE.json's 1e-3 bar END TO END (G, D, R1);
     "fp32":   every convolution runs on the exact-fp32 SIMT kernels (parity arbitration, odd shapes)."""
     global CONV_IMPL, _PRECISION
@@ -65,7 +65,7 @@ def get_precision():
 
 
 def tf32_enabled():
-    """True when operand producers should round their outputs to tf32 (kind::tf32 consumers truncate)."""
+    """True when operand producers should round their outputs to tf32 (tf32 consumers truncate)."""
     return _PRECISION == "tf32" and CONV_IMPL != 1
 
 
@@ -95,7 +95,7 @@ def _carry_planes(x, planes):
 
 
 def _tag(t, rounded):
-    """Marks a tensor whose values are exactly representable in tf32 (so a tcgen05 consumer needs no rounding pass).
+    """Marks a tensor whose values are exactly representable in tf32 (so a tensor-core consumer needs no rounding pass).
     The mark records the tensor's version counter: autograd's in-place gradient accumulation (``buffer += grad``) keeps the
     Python object -- and its attributes -- but bumps the version, which invalidates the mark."""
     if rounded:
@@ -199,7 +199,7 @@ def _wgrad_raw(x, gy, k, mode, flip, transposed, x_planes=None):
     xin, gin = x, gy
     if path == 3:                              # compensated contraction on the split planes of both operands
         xin, gin = (x_planes if x_planes is not None else _planes(x)), _planes(gy)
-    elif path == 2:                            # MN-major kind::tf32 path: operands must be tf32-representable
+    elif path == 2:                            # MN-major tf32 path: operands must be tf32-representable
         if not _is_tf32(x):
             xin = _round_tf32_raw(x)
         if not _is_tf32(gy):

@@ -1,4 +1,4 @@
-/* gifb200.h -- C ABI of libgifb200.so: the B200 (sm_100a) kernels behind GIF's StyleGAN2 / rasteriser hot path.
+/* gifb200.h -- C ABI of libgifb200.so: the H100 (sm_90a) kernels behind GIF's StyleGAN2 / rasteriser hot path.
  *
  * Boundary rules (SURVEY.md 8b):
  *   - plain `extern "C"`, device pointers + int shapes + a `cudaStream_t` (passed as void*); no torch types;
@@ -28,7 +28,7 @@ extern "C" {
 #define GIFB200_OK 0
 #define GIFB200_E_SHAPE (-1)     /* unsupported / inconsistent shape argument                       */
 #define GIFB200_E_ALIGN (-2)     /* pointer or channel count not aligned as the kernel requires     */
-#define GIFB200_E_ARCH (-3)      /* device is not sm_100 / driver entry point missing               */
+#define GIFB200_E_ARCH (-3)      /* device is not sm_90 / driver entry point missing               */
 #define GIFB200_E_CUDA (-4)      /* CUDA runtime / driver error (message has the CUDA error string) */
 #define GIFB200_E_WORKSPACE (-5) /* workspace too small                                              */
 
@@ -57,11 +57,11 @@ long long gifb200_launch_count(void);
  * so that the adjoint (input-gradient) of every mode is another call on the SAME weight buffer:
  *     adj(S1, flip, tr) = (S1, !flip, !tr);  adj(S2, flip, tr) = (T2, flip, !tr);  adj(T2, flip, tr) = (S2, flip, !tr).
  *
- * impl: 0 = auto (tcgen05 tensor-core path when the shape qualifies, else SIMT), 1 = force SIMT fp32,
- *       2 = force tcgen05 (kind::tf32, fp32 accumulate; returns GIFB200_E_SHAPE if the shape does not qualify),
- *       3 = tcgen05 ERROR-COMPENSATED contraction ("bf16x3", fp32 accumulate): every operand is the two-term bf16
+ * impl: 0 = auto (tensor-core path when the shape qualifies, else SIMT), 1 = force SIMT fp32,
+ *       2 = force the tensor-core path (wgmma tf32, fp32 accumulate; returns GIFB200_E_SHAPE if the shape does not qualify),
+ *       3 = tensor-core ERROR-COMPENSATED contraction ("bf16x3", fp32 accumulate): every operand is the two-term bf16
  *           expansion v = hi + lo written by gifb200_split_bf16 and the kernel accumulates hi*hi + hi*lo + lo*hi into the
- *           same TMEM accumulator (16 significant operand bits, ~1e-5 relative; 1.5x the tensor work of kind::tf32).
+ *           same fp32 accumulator (16 significant operand bits, ~1e-5 relative; 1.5x the tensor work of tf32).
  *           With impl 3, `x` is NOT an fp32 tensor but the planes buffer of gifb200_split_bf16 for the input
  *           (2 x B*Hi*Wi*Ci bf16 = the same number of bytes); w stays fp32 (split while staging).  Same shapes as impl 2.
  * workspace: gifb200_conv2d_workspace_bytes(...) bytes of device memory (may be 0 / NULL): the staged B operand, followed --
@@ -87,7 +87,7 @@ int gifb200_conv2d(const float* x, const float* w, float* y, int B, int Hi, int 
  *     gW[t,o,i] = sum_{b,pixels} gy[b,p_out,o] * x[b,p_in(p_out,t),i]   (p_in as in the mode's formula above)
  * x is the conv input (B,Hi,Wi,Ci), gy the conv output gradient (B,Ho,Wo,Co).  gw is OVERWRITTEN.
  * Replaces autograd's conv weight gradient for the reference modules listed above.
- * impl: 0 auto, 1 SIMT fp32, 2 tcgen05 kind::tf32 on the channels-last operands (MN-major tiles), 3 = bf16x3 compensated
+ * impl: 0 auto, 1 SIMT fp32, 2 wgmma tf32 on the channels-last operands (MN-major tiles), 3 = bf16x3 compensated
  * contraction: BOTH x and gy are planes buffers of gifb200_split_bf16 (see gifb200_conv2d). */
 size_t gifb200_conv2d_wgrad_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, int Wo, int Co, int k, int mode,
                                             int impl);
@@ -122,7 +122,7 @@ int gifb200_upfirdn2d(const float* x, const float* kernel, float* y, int B, int 
  *     t = x[b,p,c] * rowscale[b,c] + add[b,p,c] + bias[c];   y = (t > 0 ? t : slope*t) * gain
  * rowscale, add, bias may each be NULL.  rows = B*P pixels in total, P pixels per sample.
  * round_tf32 (here and below): != 0 rounds the OUTPUT to tf32 (round-to-nearest-away, cvt.rna) -- set by the caller
- * when the consumer is a tcgen05 kind::tf32 contraction, which truncates its operands: pre-rounded operands make
+ * when the consumer is a wgmma tf32 contraction, which truncates its operands: pre-rounded operands make
  * that truncation exact and the contraction unbiased. */
 int gifb200_bias_act(const float* x, const float* rowscale, const float* add, const float* bias, float* y, int B,
                      int P, int C, float slope, float gain, int round_tf32, gifb200_stream_t stream);
@@ -134,7 +134,7 @@ int gifb200_act_bwd(const float* gy, const float* y, float* gx, long long n, flo
 int gifb200_rows_sum(const float* x, float* out, int G, int rows, int C, gifb200_stream_t stream);
 /* y[b,p,c] = x[b,p,c] * s[b,c]  -- style modulation of the conv INPUT (cl.py:311-312 moved to the activation),
  * demodulation of the conv OUTPUT (cl.py:315-316).  round_tf32 != 0 rounds y to tf32 (round-to-nearest) so that
- * the tcgen05 kind::tf32 contraction, which truncates, sees exactly representable operands. */
+ * the wgmma tf32 contraction, which truncates, sees exactly representable operands. */
 int gifb200_chan_scale(const float* x, const float* s, float* y, int B, int P, int C, int round_tf32,
                        gifb200_stream_t stream);
 /* Fused first-order backward passes (used when no second derivative is requested; the composable primitives above remain

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """TEST INFRASTRUCTURE ONLY (build container) -- goldens for the TENSOR-CORE shapes of the contraction operators.
 
-``tests/golden/modconv.npz`` / ``ops.npz`` hold small shapes (Co = 16, Ci = 16 ...) that the tcgen05 kernels do not take, so
+``tests/golden/modconv.npz`` / ``ops.npz`` hold small shapes (Co = 16, Ci = 16 ...) that the tensor-core kernels do not take, so
 they pin the exact-fp32 SIMT path only.  This script evaluates the UNMODIFIED reference modules (oracle/ref_import.py) on
 shapes the tensor-core path DOES take -- channels multiples of 32, power-of-two site grids, incl. the north-star layer
 ModulatedConv2d(128,128,3) at 256^2 and BASELINE.json configs[0] -- in float64 (the truth the 1e-3 bar is read against)

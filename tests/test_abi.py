@@ -48,11 +48,11 @@ def test_error_codes_without_gpu():
 
 def test_dispatch_queries_and_one_wave_split_count():
     """Host logic that needs no GPU: which path a shape takes, workspace sizes, and that the weight-gradient kernel's grid
-    (128-channel tiles x kernel rows x pixel splits, ONE CTA per SM) never exceeds the 148 SMs -- a second wave of a few
-    straggler CTAs once doubled that kernel's time (profiles/r01_ncu_wgrad_halo_northstar_run33.md)."""
+    (128-channel tiles x kernel rows x pixel splits, ONE CTA per SM) never exceeds the 132 SMs of an H100 SXM -- a second
+    wave of a few straggler CTAs doubles that kernel's time."""
     from gif_b200 import _lib
     lib = _lib.lib
-    bn = lambda c: 128 if c % 128 == 0 else 64 if c % 64 == 0 else 32
+    bn = lambda c: 64 if c % 64 == 0 else 32
     for (B, H, Ci, Co, mode) in [(32, 256, 128, 128, 0), (32, 128, 256, 256, 0), (32, 64, 512, 512, 0), (32, 32, 512, 512, 0),
                                  (32, 257, 128, 256, 1), (32, 129, 256, 512, 1), (32, 128, 256, 128, 2), (32, 64, 512, 256, 2),
                                  (16, 256, 128, 128, 0), (8, 64, 512, 512, 0)]:
@@ -63,10 +63,10 @@ def test_dispatch_queries_and_one_wave_split_count():
         splits = wws // (9 * Co * Ci * 4)
         small, big = (Ci, Co) if mode == 2 else (Co, Ci)
         ctas = (small // 128) * (big // bn(big)) * 3 * splits
-        assert 1 <= splits and 96 <= ctas <= 148, (B, H, Ci, Co, mode, splits, ctas)
+        assert 1 <= splits and 96 <= ctas <= 132, (B, H, Ci, Co, mode, splits, ctas)
     # shapes outside the tensor-core path: exact fp32 kernels, no workspace
     assert lib.gifb200_conv2d_wgrad_path(32, 256, 256, 9, 256, 256, 128, 3, 0, 0) == 1
-    assert lib.gifb200_conv2d_wgrad_path(32, 256, 256, 9, 256, 256, 128, 3, 0, 2) == 0        # forcing tcgen05 is refused
+    assert lib.gifb200_conv2d_wgrad_path(32, 256, 256, 9, 256, 256, 128, 3, 0, 2) == 0        # forcing the tensor-core path is refused
     assert lib.gifb200_conv2d_workspace_bytes(32, 250, 250, 128, 250, 250, 128, 3, 0, 0, 0) == 0   # ragged size -> SIMT
     assert lib.gifb200_flame_lbs_workspace_bytes(64, 5) == 64 * (36 + 60) * 4
     rc = lib.gifb200_flame_lbs(None, None, None, None, None, None, None, None, None, None, None, 4, 5023, 150, 9, None, 0, None)

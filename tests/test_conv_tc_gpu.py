@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (kind::tf32) implicit-GEMM convolution against the exact-fp32 SIMT kernel through the C ABI
+"""GPU: the wgmma (tf32) implicit-GEMM convolution against the exact-fp32 SIMT kernel through the C ABI
 (impl=2 vs impl=1), every mode / flag combination, tile-edge shapes (4x4 images packed 8 per tile, batch not a multiple of
 the images-per-tile, ...).  Inputs are pre-rounded to tf32 so the only difference is the accumulation order: the bar is 2e-5
 for those, and 1e-3 (BASELINE.json) for raw fp32 inputs through gif_b200.ops (which rounds)."""
@@ -151,9 +151,9 @@ def test_wgrad_tc_matches_simt(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transpose
 
 # ------------------------------------------------------------------------------------------------ bf16x3 (compensated)
 # The error-compensated mode (gifb200_conv2d / _wgrad impl 3): UNROUNDED fp32 operands, split into two bf16 terms by
-# gifb200_split_bf16, hi*hi + hi*lo + lo*hi on kind::f16, fp32 accumulate.  Expected error ~2^-17 per operand (the dropped
+# gifb200_split_bf16, hi*hi + hi*lo + lo*hi on bf16, fp32 accumulate.  Expected error ~2^-17 per operand (the dropped
 # lo*lo term and the rounding of lo): the bar is 5e-5 against the exact-fp32 SIMT kernel on the same raw inputs -- 20x
-# inside BASELINE.json's 1e-3 and 6x inside what kind::tf32 can do (3e-4).
+# inside BASELINE.json's 1e-3 and 6x inside what tf32 can do (3e-4).
 def test_split_bf16_planes(cuda):
     from gif_b200 import ops
     x = torch.randn(3, 5, 7, 32, device=cuda) * 3.0

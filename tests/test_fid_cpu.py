@@ -1,9 +1,6 @@
 """Evaluation path (SURVEY 8f.4): Frechet distance and streaming activation statistics against the reference's formulas
 (my_utils/pytorch_fid/fid_score.py:142-196 = scipy sqrtm of the covariance product; compute_fid.py:79-80 = np.mean / np.cov),
-and -- when the reference tree is present -- against the reference's own function."""
-import os
-import sys
-
+and against the stored result of the reference's own function."""
 import numpy as np
 import pytest
 import torch
@@ -30,21 +27,12 @@ def test_frechet_distance_matches_sqrtm_form(d, n):
 
 
 def test_frechet_distance_matches_reference_function_live():
-    path = "/root/reference/my_utils/pytorch_fid/fid_score.py"
-    if not os.path.isfile(path):
-        pytest.skip("reference tree not present (container-only check)")
-    src = open(path).read()
-    start, end = src.index("def calculate_frechet_distance"), src.index("def calculate_activation_statistics")
-    import types
-    # scipy >= 1.15 dropped sqrtm's ``disp`` argument the reference still passes (fid_score.py:176): restore the old
-    # calling convention (disp=False returns (sqrtm, error estimate)) around the same scipy routine
-    compat = types.SimpleNamespace(sqrtm=lambda a, disp=True: linalg.sqrtm(a) if disp else (linalg.sqrtm(a), 0.0))
-    ns = {"np": np, "linalg": compat}
-    exec(compile(src[start:end], path, "exec"), ns)          # the unmodified function, without the module's torchvision imports
-    rng = np.random.default_rng(5)
-    a, b = rng.normal(size=(400, 96)), rng.normal(size=(400, 96)) @ rng.normal(size=(96, 96)) * 0.2
-    m1, s1, m2, s2 = a.mean(0), np.cov(a, rowvar=False), b.mean(0), np.cov(b, rowvar=False)
-    want = ns["calculate_frechet_distance"](m1, s1, m2, s2)
+    """The reference's own calculate_frechet_distance (fid_score.py:142-196) on seeded statistics; its result is stored in
+    tests/golden/reference_live.npz (oracle/make_live_golden.py)."""
+    import golden_util as gu
+    import live_cases
+    want = float(gu.load_golden("reference_live.npz")["fid_reference"][0])
+    m1, s1, m2, s2 = live_cases.fid_case()
     assert abs(fid.calculate_frechet_distance(m1, s1, m2, s2, device=torch.device("cpu")) - want) < 1e-7 * abs(want)
 
 

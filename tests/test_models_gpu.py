@@ -1,7 +1,7 @@
 """GPU parity tests of the generator / discriminator / R1 / PPL against the reference goldens and the oracle, in the
-three precision modes of gif_b200.ops (measured table: profiles/r02_precision_report.jsonl, tools/precision_report.py):
+three precision modes of gif_b200.ops (tools/precision_report.py measures the table):
 
-    quantity (vs reference golden)        fp32 SIMT    tf32 tcgen05    bf16x3 tcgen05      bar of BASELINE.json
+    quantity (vs reference golden)        fp32 SIMT    tf32 wgmma      bf16x3 wgmma        bar of BASELINE.json
     G 32^2 / 256^2 forward (max-rel)      3.5e-6       0.9-1.2e-3      4.7e-5 / 8.8e-5     1e-3
     D 64^2 / 256^2 scores                 1.4e-6       6.1e-4          3.9e-5 / 6.1e-5     1e-3
     R1 penalty (double backward)          3.1e-5       1.3e-2          3.3e-4              1e-3

@@ -3,8 +3,8 @@
 reference's own fp32-vs-fp64 floor), in every precision mode of gif_b200.ops:
 
     mode      kernel                                       bar, forward      bar, first derivatives
-    tf32      tcgen05 kind::tf32                           1e-3              max(1e-3, 3 x fp32 floor); 5e-2 THROUGH leaky ReLUs
-    bf16x3    tcgen05 kind::f16, hi*hi + hi*lo + lo*hi     1e-4              max(1e-4, 3 x fp32 floor)
+    tf32      wgmma tf32                           1e-3              max(1e-3, 3 x fp32 floor); 5e-2 THROUGH leaky ReLUs
+    bf16x3    wgmma bf16, hi*hi + hi*lo + lo*hi     1e-4              max(1e-4, 3 x fp32 floor)
     fp32      SIMT fp32                                    2e-5              max(2e-5, 3 x fp32 floor)
 
 The bar of BASELINE.json is 1e-3 relative to fp32; both the max-norm relative error (golden_util.rel_err) and the
@@ -58,7 +58,7 @@ def _check(tag, names, tensors, g, tol, report, grad_tol=None, l2_only=None):
 def _assert_tensor_core(B, H, W, ci, co, k, mode_id=0):
     from gif_b200._lib import lib
     ho = H if mode_id == 0 else ((H - k) // 2 + 1 if mode_id == 1 else 2 * (H - 1) + k)
-    assert lib.gifb200_conv2d_workspace_bytes(B, H, W, ci, ho, ho, co, k, mode_id, 0, 2) > 0, "shape not on the tcgen05 path"
+    assert lib.gifb200_conv2d_workspace_bytes(B, H, W, ci, ho, ho, co, k, mode_id, 0, 2) > 0, "shape not on the tensor-core path"
 
 
 @pytest.mark.parametrize("mode,tol", MODES)
@@ -138,7 +138,7 @@ def test_res_block_tc_shapes(cuda, gold, mode, tol):
         grads = torch.autograd.grad((y * gy).sum(), [x] + [named[n] for n in pn])
         rep = []
         # gradients THROUGH the two leaky ReLUs: a forward error eps flips ~eps of the masks, i.e. an L2 gradient error
-        # ~sqrt(eps) (tests/test_models_gpu.py docstring).  kind::tf32 (eps ~3e-4) cannot hold 1e-3 here -- measured 3.3e-2,
+        # ~sqrt(eps) (tests/test_models_gpu.py docstring).  tf32 (eps ~3e-4) cannot hold 1e-3 here -- measured 3.3e-2,
         # bar 5e-2, which is why tf32 is not the headline mode; bf16x3 (5.8e-6 measured) and fp32 keep the forward bar.
         _check("rb", ["y", "gx"] + ["g_" + n for n in pn], [y] + list(grads), gold, 2 * tol, rep,
                grad_tol=5e-2 if mode == "tf32" else None)

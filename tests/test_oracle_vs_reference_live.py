@@ -1,16 +1,19 @@
-"""CPU, container-only: the oracle restatement against the LIVE unmodified reference modules over randomised
-configurations (the committed goldens pin fixed cases; this sweeps shapes, pads, flags).  fp64 where the reference allows it
-(its make_kernel is fp32-only: cl.py:83-91), bar 1e-11; skipped where /root/reference does not exist (the GPU box)."""
-import math
-
+"""CPU: the oracle restatement against the unmodified reference modules over randomised configurations (the other goldens
+pin fixed cases; this sweeps shapes, pads, flags).  The reference's outputs for these seeded inputs are stored in
+tests/golden/reference_live.npz (oracle/make_live_golden.py; inputs: tests/live_cases.py).  fp64 where the reference allows
+it (its make_kernel is fp32-only: cl.py:83-91), bar 1e-11."""
 import pytest
 import torch
 
-from oracle import ref_import
+import golden_util as gu
+import live_cases as LC
 from oracle import stylegan2_oracle as O
 
-pytestmark = pytest.mark.skipif(not ref_import.available(), reason="reference tree not present (GPU box)")
 DT = torch.float64
+
+
+def _g(key):
+    return torch.from_numpy(gu.load_golden("reference_live.npz")[key])
 
 
 def _close(a, b, tol=1e-11):
@@ -21,66 +24,33 @@ def _close(a, b, tol=1e-11):
 
 @pytest.mark.parametrize("seed", range(6))
 def test_upfirdn2d_random_configs(seed):
-    R = ref_import.load()
-    g = torch.Generator().manual_seed(seed)
-    for _ in range(6):
-        up, down = int(torch.randint(1, 3, (1,), generator=g)), int(torch.randint(1, 3, (1,), generator=g))
-        p0, p1 = int(torch.randint(-1, 4, (1,), generator=g)), int(torch.randint(0, 4, (1,), generator=g))
-        h, w = int(torch.randint(5, 14, (1,), generator=g)), int(torch.randint(5, 14, (1,), generator=g))
-        kh = int(torch.randint(2, 5, (1,), generator=g))
-        k = torch.randn(kh, kh, generator=g, dtype=DT)
-        x = torch.randn(2, 3, h, w, generator=g, dtype=DT)
-        if (h * up + p0 + p1 - kh) // down + 1 <= 0 or (w * up + p0 + p1 - kh) // down + 1 <= 0:
-            continue
-        _close(O.upfirdn2d(x, k, up, down, (p0, p1)), R.cl.upfirdn2d(x, k, up=up, down=down, pad=(p0, p1)))
+    cases = LC.upfirdn_cases(seed)
+    assert cases
+    for j, (x, k, up, down, pad) in enumerate(cases):
+        _close(O.upfirdn2d(x, k, up, down, pad), _g(f"upfirdn_{seed}_{j}"))
 
 
 @pytest.mark.parametrize("seed", range(4))
 @pytest.mark.parametrize("upsample", [False, True])
 @pytest.mark.parametrize("demod", [True, False])
 def test_modulated_conv2d_random_configs(seed, upsample, demod):
-    R = ref_import.load()
-    g = torch.Generator().manual_seed(100 + seed)
-    ci, co = int(torch.randint(2, 9, (1,), generator=g)), int(torch.randint(2, 9, (1,), generator=g))
-    k = 3 if upsample or seed % 2 == 0 else 1
-    r, b, sdim = int(torch.randint(3, 8, (1,), generator=g)), int(torch.randint(1, 4, (1,), generator=g)), 7
-    with ref_import.quiet():
-        m = R.cl.ModulatedConv2d(ci, co, k, sdim, demodulate=demod, upsample=upsample).double()
-    if upsample:
-        m.blur.kernel = m.blur.kernel.double()
-    m.weight.data = torch.randn(m.weight.shape, generator=g, dtype=DT)
-    m.modulation.weight.data = torch.randn(m.modulation.weight.shape, generator=g, dtype=DT)
-    m.modulation.bias.data = torch.randn(m.modulation.bias.shape, generator=g, dtype=DT)
-    x = torch.randn(b, ci, r, r, generator=g, dtype=DT)
-    s = torch.randn(b, sdim, generator=g, dtype=DT)
-    y_o = O.modulated_conv2d(x, s, m.weight.data, m.modulation.weight.data, m.modulation.bias.data, demodulate=demod,
-                             upsample=upsample, blur_kernel=m.blur.kernel if upsample else None)
-    _close(y_o, m(x, s))
+    c = LC.modconv_case(seed, upsample, demod)
+    key = f"modconv_{seed}_{int(upsample)}_{int(demod)}"
+    y_o = O.modulated_conv2d(c["x"], c["s"], c["weight"], c["mod_weight"], c["mod_bias"], demodulate=demod,
+                             upsample=upsample, blur_kernel=_g(key + "_blur") if upsample else None)
+    _close(y_o, _g(key))
 
 
 @pytest.mark.parametrize("seed", range(4))
 def test_equal_layers_random_configs(seed):
-    R = ref_import.load()
-    g = torch.Generator().manual_seed(200 + seed)
-    i, o = int(torch.randint(2, 20, (1,), generator=g)), int(torch.randint(2, 20, (1,), generator=g))
-    for act, lr_mul in ((None, 1.0), ("fused_lrelu", 0.01), (None, 0.5)):
-        with ref_import.quiet():
-            m = R.cl.EqualLinear(i, o, bias_init=0.3, lr_mul=lr_mul, activation=act).double()
-        m.weight.data = torch.randn(o, i, generator=g, dtype=DT) / lr_mul
-        x = torch.randn(5, i, generator=g, dtype=DT)
-        _close(O.equal_linear(x, m.weight.data, m.bias.data, lr_mul=lr_mul, activation=act is not None), m(x))
-    for k, stride, pad, r in ((1, 1, 0, 6), (3, 1, 1, 6), (3, 2, 0, 9), (1, 2, 0, 7)):
-        with ref_import.quiet():
-            c = R.cl.EqualConv2d(i, o, k, stride=stride, padding=pad).double()
-        c.weight.data = torch.randn(c.weight.shape, generator=g, dtype=DT)
-        c.bias.data = torch.randn(o, generator=g, dtype=DT)
-        x = torch.randn(2, i, r, r, generator=g, dtype=DT)
-        _close(O.equal_conv2d(x, c.weight.data, c.bias.data, stride=stride, padding=pad), c(x))
-    f = R.cl.FusedLeakyReLU(o).double()
-    f.bias.data = torch.randn(f.bias.shape, generator=g, dtype=DT)
-    x = torch.randn(3, o, 4, 5, generator=g, dtype=DT)
-    _close(O.fused_leaky_relu(x, f.bias.data), f(x))
-    _close(O.pixel_norm(x), R.cl.PixelNorm()(x))
+    lin, conv, (x, bias, o) = LC.equal_cases(seed)
+    for j, (xl, w, i, o_, act, lr_mul) in enumerate(lin):
+        _close(O.equal_linear(xl, w, _g(f"equal_linear_{seed}_{j}_bias"), lr_mul=lr_mul, activation=act is not None),
+               _g(f"equal_linear_{seed}_{j}"))
+    for j, (xc, w, b, i, o_, k, stride, pad) in enumerate(conv):
+        _close(O.equal_conv2d(xc, w, b, stride=stride, padding=pad), _g(f"equal_conv_{seed}_{j}"))
+    _close(O.fused_leaky_relu(x, bias), _g(f"fused_lrelu_{seed}"))
+    _close(O.pixel_norm(x), _g(f"pixel_norm_{seed}"))
 
 
 def test_condition_pyramid_equals_bilinear_interpolate():
@@ -94,27 +64,18 @@ def test_condition_pyramid_equals_bilinear_interpolate():
 
 
 def test_minibatch_stddev_and_r1_against_reference_discriminator_tail():
-    """disc.py:59-65 (group statistics) through a whole small discriminator in fp64, incl. the R1 penalty's double backward."""
-    import golden_util as gu
-    R = ref_import.load()
-    with ref_import.quiet():
-        D = R.disc.Discriminator(size=16, num_color_chnls=9, channel_multiplier=2).double()
-    sd = {k: v.double() for k, v in gu.seeded_state_dict(gu.d_shapes(16), 31).items()}
-    D.load_state_dict(sd)
-    for mod in D.modules():                       # the FIR buffers are created fp32 (cl.py:83-91)
-        if hasattr(mod, "kernel") and torch.is_tensor(mod.kernel):
-            mod.kernel = mod.kernel.double()
-    img = gu.rand_uniform((8, 3, 16, 16), 32).double().requires_grad_(True)
-    cond = gu.rand_uniform((8, 6, 16, 16), 33).double()
-    s_ref, _ = D([img], condition=cond, step=2, alpha=1)
-    pen_ref = R.losses.grad_penalty_loss([img], s_ref, step=None)
-    (g_ref,) = torch.autograd.grad(pen_ref.mean(), D.final_linear[0].weight)
-    img2 = img.detach().clone().requires_grad_(True)
+    """disc.py:59-65 (group statistics) through a whole small discriminator in fp64, incl. the R1 penalty's double backward
+    (its weight gradient compared on a fixed sample of positions, normalised by the full gradient's largest magnitude)."""
+    sd, img, cond = LC.disc_tail_case()
+    img2 = img.clone().requires_grad_(True)
     sdo = {k: v.clone() for k, v in sd.items()}
     sdo["final_linear.0.weight"].requires_grad_(True)
     s_o = O.discriminator_forward(img2, cond, sdo, 16)
     pen_o = O.r1_penalty(s_o, img2)
     (g_o,) = torch.autograd.grad(pen_o.mean(), sdo["final_linear.0.weight"])
-    _close(s_o, s_ref)
-    _close(pen_o, pen_ref)
-    _close(g_o, g_ref, 1e-9)
+    _close(s_o, _g("disc_scores"))
+    _close(pen_o, _g("disc_r1"))
+    g_s = g_o.reshape(-1)[LC.grad_sample_index(g_o.numel())]
+    err = float((g_s - _g("disc_r1_grad_sample")).abs().max()) / float(_g("disc_r1_grad_absmax")[0])
+    assert err < 1e-9, err
+    assert abs(float(g_o.abs().max()) - float(_g("disc_r1_grad_absmax")[0])) <= 1e-9 * float(_g("disc_r1_grad_absmax")[0])

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Measures the tensor-pipe roofline denominator for the MMA kind the convolutions use (kind::tf32): cuBLAS fp32 GEMM with
+"""Measures the tensor-pipe roofline denominator for the MMA kind the convolutions use (tf32): cuBLAS fp32 GEMM with
 TF32 tensor cores allowed, 8192^3, as a burst (best of 10, a kernel timed alone) and sustained (back to back for 4 s, a
 kernel timed inside a long step) -- the same protocol MEASURED_PEAKS.json documents for its bf16 entry.  Also the
 3xTF32-equivalent ceiling (one third of it) and the plain fp32 SIMT rate for context.
-Prints one JSON line; bench.py reads profiles/r02_tf32_peak.json (a committed copy of that line)."""
+Prints one JSON line."""
 import json
 import time
 

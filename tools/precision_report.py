@@ -2,7 +2,7 @@
 """Measured deviation from the reference goldens per precision mode (fp32 SIMT / tf32 / bf16x3), network level:
 generator 32^2 forward + gradients, generator 256^2 forward, discriminator 64^2 scores + R1 penalty + gradients,
 discriminator 256^2 scores.  Prints one JSON line per (mode, quantity); the bars of tests/test_models_gpu.py and of
-__graft_entry__.smoke() are set from this table (profiles/r02_precision_report.jsonl)."""
+__graft_entry__.smoke() are set from this table."""
 import json
 import math
 import os
