@@ -1,7 +1,7 @@
 // wgmma implicit-GEMM convolution for sm_90a (tf32 operands, fp32 accumulation in registers).
 //
 // GEMM view (per output "phase"):  D[site, o] = sum_{tap} sum_{i} A_tap[site, i] * W[tap][o][i]
-//   M = 128 sites per CTA (a wt x ht x nt box of the site grid (B, Hs, Ws)), N = BLOCK_N output channels,
+//   M = BM sites per CTA (a wt x ht x nt box of the site grid (B, Hs, Ws)), N = BN output channels (see TileCfg),
 //   K = 32 input channels per pipeline stage (one 128-byte swizzle row of fp32), taps x Ci/32 stages per tile.
 //   * A operand: the activation tensor itself (channels-last fp32) -- no im2col buffer.  Each tap is the same TMA box
 //     shifted by the tap offset; TMA's out-of-bounds zero fill implements the padding.  Stride-2 convolutions (S2)
@@ -10,11 +10,12 @@
 //     subset of the 9 taps, and write with output stride 2.
 //   * B operand: the tap-major weights [T][Co][Ci] staged once per call into the workspace (honouring flip /
 //     transposed, rounded to tf32), K-major, 128B swizzle.
-//   * Both operands are K-major SWIZZLE_128B; each of two consumer warpgroups issues one wgmma.m64nNk8.tf32 (its 64 rows
-//     of the tile, N = BLOCK_N) per 32-byte K slice; accumulators live in registers (BLOCK_N / 2 per thread).
-//   * Warp roles (288 threads): warps 0-7 two consumer warpgroups (MMA + fused epilogue from registers, 8-byte global
-//     stores, channels-last), warp 8 TMA producer.
-//   * 3-stage smem ring (96 KB) so that two CTAs share an SM: one CTA's epilogue overlaps the other's main loop.
+//   * Both operands are K-major SWIZZLE_128B; each of two consumer warpgroups issues one wgmma.m64nNk8.tf32 per m64 row
+//     block of its BM/2 rows (N = BN) per 32-byte K slice; accumulators live in registers (BM * BN / 256 per thread).
+//   * Warp roles: warps 0-7 two consumer warpgroups (MMA + fused epilogue from registers, 8-byte global stores,
+//     channels-last), warp 8 TMA producer.
+//   * 128 x BN tiles: 3-stage smem ring (96 KB) so that two CTAs share an SM: one CTA's epilogue overlaps the other's main
+//     loop.  Large tiles (128 x 256, 256 x 128): one CTA per SM, 4-stage ring (192 KB), register reallocation.
 //
 // Operand precision: the tf32 MMA reads the upper 19 bits of each fp32 (truncation).  Callers hand in activations that
 // are already rounded to tf32 (gif_b200.ops rounds in the producing kernel), weights are rounded here, so the
@@ -22,7 +23,7 @@
 //
 // X3 = true is the error-compensated mode ("bf16x3", gifb200_conv2d impl 3): operands arrive as two bf16 planes (hi, lo)
 // per tensor (gifb200_split_bf16; the weights are split while staging), a stage holds the hi and the lo tile of A and of B
-// as K-major SWIZZLE_64B tiles of 32 channels (128 rows x 64 B: the SAME number of bytes per stage as the fp32 tiles), and
+// as K-major SWIZZLE_64B tiles of 32 channels (rows of 64 B: the SAME number of bytes per stage as the fp32 tiles), and
 // each 16-channel slice issues three bf16 wgmmas -- lo*hi, hi*lo, hi*hi -- into the one fp32 register accumulator.
 // Everything else (tile walk, ring, epilogue) is shared with the tf32 kernel.
 #include <cuda_bf16.h>
@@ -33,17 +34,13 @@ namespace gifb200 {
 
 namespace {
 
-constexpr int kStages = 3;
-constexpr int kBlockM = 128;
 constexpr int kBlockK = 32;                         // fp32 elements = 128 bytes = one swizzle row
-constexpr int kATileBytes = kBlockM * kBlockK * 4;  // 16 KB
 constexpr int kMaxTaps = 9;
-constexpr int kConsumerWarps = 8;                   // two warpgroups: rows 0-63 and 64-127 of the tile
-constexpr int kTcThreads = 32 * kConsumerWarps + 32;   // + one TMA producer warp
+constexpr int kConsumerWarps = 8;                   // two warpgroups: the upper and the lower half of the tile's rows
 
 struct TcParams {
     int B, Hs, Ws;          // site grid per image
-    int wt, ht, nt;         // tile box (wt*ht*nt == 128)
+    int wt, ht, nt;         // tile box (wt*ht*nt == BM)
     int tiles_x, tiles_y;   // tiles per image group
     int Ci, Co;
     int s2;                 // 1: A loads go through the 5-D parity view, one site row per TMA issue
@@ -62,13 +59,30 @@ struct TcParams {
     ConvEpilogue epi;
 };
 
-template <int BLOCK_N>
-struct SmemLayout {
-    static constexpr int kBTileBytes = BLOCK_N * kBlockK * 4;
+// CTA tile of BM sites x BN output channels.  Two shapes of the same kernel:
+//  * 128 x BN (BN <= 128): 288 threads (two consumer warpgroups + one producer warp), 3-stage ring of 32 KB stages,
+//    two CTAs per SM (<= 112 registers per thread: 64 accumulators);
+//  * large, 128 x 256 or 256 x 128: 384 threads (two consumer warpgroups + a producer warpgroup), one CTA per SM, 4-stage
+//    ring of 48 KB stages; setmaxnreg moves the producer warpgroup down to 40 registers and the consumers up to 232
+//    (128 accumulators).  Per MAC the larger tile loads 3/4 of the TMA bytes of a 128 x 128 tile, and 128 x 256 also
+//    reads its A operand from shared memory half as often.
+// Each consumer warpgroup owns BM/2 rows of the tile as BM/128 m64 row blocks.
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // large tiles: 128 * 40 + 256 * 232 <= 65536 registers per SM
+template <int BM, int BN>
+struct TileCfg {
+    static constexpr bool kLarge = BM * BN > 128 * 128;
+    static constexpr int kRowBlocks = BM / 128;
+    static constexpr int kAcc = kRowBlocks * BN / 2;      // fp32 accumulators per consumer thread
+    static constexpr int kStages = kLarge ? 4 : 3;
+    static constexpr int kThreads = kLarge ? 384 : 32 * kConsumerWarps + 32;
+    static constexpr int kMinBlocks = kLarge ? 1 : 2;
+    static constexpr int kATileBytes = BM * kBlockK * 4;
+    static constexpr int kBTileBytes = BN * kBlockK * 4;
     static constexpr int kStageBytes = kATileBytes + kBTileBytes;
     static constexpr int kBarrierOffset = kStages * kStageBytes;
-    static constexpr int kTotal = kBarrierOffset + 64;    // full[3], empty[3]
-    static constexpr int kDynamic = kTotal + 1024;        // slack for manual 1024 B alignment
+    static constexpr int kTotal = kBarrierOffset + 16 * kStages;    // full[kStages], empty[kStages]
+    static constexpr int kDynamic = kTotal + 1024;                  // slack for manual 1024 B alignment
+    static_assert(kDynamic <= 227 * 1024, "shared memory ring too large");
 };
 
 // Tile order: (output-channel block, phase) vary FASTEST, the site tile slowest, so that the CTAs running at the same
@@ -83,25 +97,26 @@ __device__ __forceinline__ void decode_tile(int tile, int nblocks, int nphase, i
     phase = nphase == 1 ? 0 : (rem / nblocks + mt / rot_div) % nphase;
 }
 
-// Persistent: gridDim.x CTAs (<= 2 per SM) walk the tile list (see decode_tile).  Warps 0-7 are two consumer warpgroups
-// (wgmma into register accumulators, then the fused epilogue straight from registers), warp 8 is the TMA producer.  The
-// smem ring and its phase bits run continuously across tiles; the second resident CTA overlaps its main loop with this
-// CTA's epilogue.
-template <int BLOCK_N, bool X3>
-__global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_constant__ CUtensorMap map_a,
-                                                         const __grid_constant__ CUtensorMap map_a2,
-                                                         const __grid_constant__ CUtensorMap map_b,
-                                                         const __grid_constant__ CUtensorMap map_b2,
-                                                         float* __restrict__ y, const TcParams p, const int mtiles,
-                                                         const int total_tiles) {
-    using L = SmemLayout<BLOCK_N>;
+// Persistent: gridDim.x CTAs (TileCfg::kMinBlocks per SM) walk the tile list (see decode_tile).  Warps 0-7 are two consumer
+// warpgroups (wgmma into register accumulators, then the fused epilogue straight from registers), warp 8 is the TMA
+// producer (large tiles: warps 9-11 complete its warpgroup for setmaxnreg and then leave).  The smem ring and its phase
+// bits run continuously across tiles, so the producer fills the next tile's first stages while the consumers store; with
+// 128 x BN tiles the second resident CTA also overlaps its main loop with this CTA's epilogue.
+template <int BM, int BN, bool X3>
+__global__ void __launch_bounds__(TileCfg<BM, BN>::kThreads, TileCfg<BM, BN>::kMinBlocks)
+    conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_a2,
+                   const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_b2,
+                   float* __restrict__ y, const TcParams p, const int mtiles, const int total_tiles) {
+    using L = TileCfg<BM, BN>;
+    constexpr int kStages = L::kStages;
+    constexpr int kATileBytes = L::kATileBytes;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarrierOffset);
     uint64_t* empty_bar = full_bar + kStages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nblocks = p.Co / BLOCK_N;
+    const int nblocks = p.Co / BN;
     const int kchunks = p.Ci / kBlockK;
     const int rot_div = max(1, static_cast<int>(gridDim.x) / (nblocks * p.nphase));
     (void)mtiles;
@@ -119,7 +134,9 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
     }
     __syncthreads();
 
-    if (warp == kConsumerWarps) {
+    if (warp >= kConsumerWarps) {
+        if constexpr (L::kLarge) setmaxnreg_dec<kProducerRegs>();
+        if (warp != kConsumerWarps) return;
         // ===================== TMA producer =====================
         // Lane 0 owns the barriers.  In stride-2 row mode the A tile is nt*ht separate row boxes (the parity view cannot be
         // one box): the 32 lanes issue them in parallel.
@@ -172,24 +189,26 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
                     }
                 }
                 if (lane == 0) {
-                    tma_load_3d(b_dst, &map_b, &full_bar[stage], c0, nblk * BLOCK_N, p.tap_w[phase][tap]);
-                    if (X3) tma_load_3d(b_dst + L::kBTileBytes / 2, &map_b2, &full_bar[stage], c0, nblk * BLOCK_N, p.tap_w[phase][tap]);
+                    tma_load_3d(b_dst, &map_b, &full_bar[stage], c0, nblk * BN, p.tap_w[phase][tap]);
+                    if (X3) tma_load_3d(b_dst + L::kBTileBytes / 2, &map_b2, &full_bar[stage], c0, nblk * BN, p.tap_w[phase][tap]);
                 }
                 if (++stage == kStages) { stage = 0; ph ^= 1; }
             }
         }
     } else {
         // ===================== consumers: wgmma main loop + epilogue =====================
-        const int wg = warp >> 2;                    // rows 64*wg .. 64*wg+63 of the tile
+        if constexpr (L::kLarge) setmaxnreg_inc<kConsumerRegs>();
+        const int wg = warp >> 2;                    // rows (BM/2)*wg .. (BM/2)*(wg+1)-1 of the tile
         const int wq = warp & 3;
-        constexpr int kAcc = BLOCK_N / 2;
+        constexpr int kRB = L::kRowBlocks;
+        constexpr int kAcc = L::kAcc;                // row block rb: acc[rb * BN/2 ...] (m64nBN fragment)
         float acc[kAcc];
-        // the two rows (h = 0, 1) this thread holds in the accumulator fragment, and their place in the site box
-        int w_in[2], h_in[2], n_in[2];
+        // the two rows (h = 0, 1) per row block this thread holds in the accumulator fragment, and their place in the site box
+        int w_in[2 * kRB], h_in[2 * kRB], n_in[2 * kRB];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int r = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
-            w_in[h] = r % p.wt; h_in[h] = (r / p.wt) % p.ht; n_in[h] = r / (p.wt * p.ht);
+        for (int rh = 0; rh < 2 * kRB; ++rh) {
+            const int r = wg * (BM / 2) + (rh >> 1) * 64 + wq * 16 + (lane >> 2) + 8 * (rh & 1);
+            w_in[rh] = r % p.wt; h_in[rh] = (r / p.wt) % p.ht; n_in[rh] = r / (p.wt * p.ht);
         }
         int stage = 0;
         uint32_t ph = 0;
@@ -207,23 +226,33 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
                 fence_regs<kAcc>(acc);
                 if (X3) {
                     // v = hi + lo per operand: acc += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (the 2^-18 lo*lo term is dropped);
-                    // small terms first.  K = 16 bf16 = 32 bytes: two slices per 32-channel stage.  A rows of 64 B.
-                    const uint32_t a_wg = a_addr + wg * 64 * 64;
-                    const uint64_t ah = make_kmajor_sw64_desc(a_wg), al = make_kmajor_sw64_desc(a_wg + kATileBytes / 2);
+                    // small terms first.  K = 16 bf16 = 32 bytes: two slices per 32-channel stage.  A rows of 64 B.  The
+                    // row blocks are independent accumulators: each keeps this per-slice order.
+                    const uint32_t a_wg = a_addr + wg * (BM / 2) * 64;
                     const uint64_t bh = make_kmajor_sw64_desc(a_addr + kATileBytes);
                     const uint64_t bl = make_kmajor_sw64_desc(a_addr + kATileBytes + L::kBTileBytes / 2);
 #pragma unroll
                     for (int k = 0; k < kBlockK / 16; ++k) {
-                        wgmma_bf16<BLOCK_N>(acc, al + 2 * k, bh + 2 * k, (it != it0) || k != 0, Trans<0>());
-                        wgmma_bf16<BLOCK_N>(acc, ah + 2 * k, bl + 2 * k, 1, Trans<0>());
-                        wgmma_bf16<BLOCK_N>(acc, ah + 2 * k, bh + 2 * k, 1, Trans<0>());
+#pragma unroll
+                        for (int rb = 0; rb < kRB; ++rb) {
+                            const uint64_t ah = make_kmajor_sw64_desc(a_wg + rb * 64 * 64);
+                            const uint64_t al = make_kmajor_sw64_desc(a_wg + rb * 64 * 64 + kATileBytes / 2);
+                            float* d = acc + rb * (BN / 2);
+                            wgmma_bf16<BN>(d, al + 2 * k, bh + 2 * k, (it != it0) || k != 0, Trans<0>());
+                            wgmma_bf16<BN>(d, ah + 2 * k, bl + 2 * k, 1, Trans<0>());
+                            wgmma_bf16<BN>(d, ah + 2 * k, bh + 2 * k, 1, Trans<0>());
+                        }
                     }
                 } else {
-                    const uint64_t adesc = make_kmajor_sw128_desc(a_addr + wg * 64 * 128);
                     const uint64_t bdesc = make_kmajor_sw128_desc(a_addr + kATileBytes);
 #pragma unroll
-                    for (int k = 0; k < kBlockK / 8; ++k)   // K = 8 tf32 = 32 bytes: advance the start address by 32 B (>>4 = 2)
-                        wgmma_tf32<BLOCK_N>(acc, adesc + 2 * k, bdesc + 2 * k, (it != it0) || k != 0);
+                    for (int k = 0; k < kBlockK / 8; ++k) {  // K = 8 tf32 = 32 bytes: advance the start address by 32 B (>>4 = 2)
+#pragma unroll
+                        for (int rb = 0; rb < kRB; ++rb) {
+                            const uint64_t adesc = make_kmajor_sw128_desc(a_addr + (wg * (BM / 2) + rb * 64) * 128);
+                            wgmma_tf32<BN>(acc + rb * (BN / 2), adesc + 2 * k, bdesc + 2 * k, (it != it0) || k != 0);
+                        }
+                    }
                 }
                 wgmma_commit();
                 fence_regs<kAcc>(acc);
@@ -241,16 +270,18 @@ __global__ void __launch_bounds__(kTcThreads, 2) conv_tc_kernel(const __grid_con
             const int tx = m % p.tiles_x; m /= p.tiles_x;
             const int ty = m % p.tiles_y; m /= p.tiles_y;
             float* base = p.ksplit > 1 ? p.part + ks * p.part_stride : y;
-            const int c0 = nblk * BLOCK_N + 2 * (lane & 3);
+            const int c0 = nblk * BN + 2 * (lane & 3);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int n = m * p.nt + n_in[h];
-                const int Y = (ty * p.ht + h_in[h]) * p.oys + p.phase_oy0[phase], X = (tx * p.wt + w_in[h]) * p.oxs + p.phase_ox0[phase];
+            for (int rh = 0; rh < 2 * kRB; ++rh) {
+                const int h = rh & 1;
+                const float* a = acc + (rh >> 1) * (BN / 2);
+                const int n = m * p.nt + n_in[rh];
+                const int Y = (ty * p.ht + h_in[rh]) * p.oys + p.phase_oy0[phase], X = (tx * p.wt + w_in[rh]) * p.oxs + p.phase_ox0[phase];
                 if (n < p.B && Y < p.Ho && X < p.Wo) {
                     float* dst = base + ((static_cast<long long>(n) * p.Ho + Y) * p.Wo + X) * p.Co + c0;
 #pragma unroll
-                    for (int j = 0; j < BLOCK_N / 8; ++j) {
-                        float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                    for (int j = 0; j < BN / 8; ++j) {
+                        float2 v = make_float2(a[4 * j + 2 * h], a[4 * j + 2 * h + 1]);
                         if (p.epi.act && p.ksplit == 1) {      // split-K: the reduction pass applies the epilogue to the sum
                             v.x = apply_epilogue(p.epi, v.x, c0 + 8 * j);
                             v.y = apply_epilogue(p.epi, v.y, c0 + 8 * j + 1);
@@ -315,10 +346,11 @@ int pick_ksplit(long long tiles, int iters, int mode) {
     return ks < 2 ? 1 : static_cast<int>(ks);
 }
 
-void tile_geometry(int B, int Hs, int Ws, int& wt, int& ht, int& nt, long long& mtiles) {
+// the wt x ht x nt site box of a bm-site tile: at most 128 sites along a row, then rows, then whole images
+void tile_geometry(int B, int Hs, int Ws, int bm, int& wt, int& ht, int& nt, long long& mtiles) {
     wt = Ws < 128 ? Ws : 128;
-    ht = (128 / wt) < Hs ? (128 / wt) : Hs;
-    nt = 128 / (wt * ht);
+    ht = (bm / wt) < Hs ? (bm / wt) : Hs;
+    nt = bm / (wt * ht);
     mtiles = static_cast<long long>(Ws / wt) * (Hs / ht) * ((B + nt - 1) / nt);
 }
 
@@ -330,6 +362,26 @@ int pick_block_n(int Co) {
     if (Co % 64 == 0) return 64;
     if (Co % 32 == 0) return 32;
     return 0;
+}
+
+// fewest large tiles (over all phases) for which a layer runs on them: with fewer, one CTA per SM leaves more than a quarter
+// of the SMs idle.  Measured on H100 (bf16x3 and tf32): 128 large tiles beat 256 128 x 128 tiles by 5-17 % (16^2 and 8^2 T2
+// layers at batch 32), 64 large tiles lose 17-24 % to 128 of them (the same layers at batch 16).
+constexpr long long kLargeMinTiles = 3 * kNumSMs / 4;
+
+// CTA tile (bm sites x bn channels) of a layer: 128 x 256 when Co % 256 == 0, else 256 x 128 when Co % 128 == 0, if the
+// layer has enough such tiles; otherwise 128 x pick_block_n(Co), which also keeps the split-K schedule.
+void pick_tile(int B, int Hs, int Ws, int Co, int nphase, int ksplit, int& bm, int& bn) {
+    bm = 128;
+    bn = pick_block_n(Co);
+    if (ksplit > 1 || Co % 128 != 0) return;
+    const int lbm = Co % 256 == 0 ? 128 : 256, lbn = Co % 256 == 0 ? 256 : 128;
+    int wt, ht, nt;
+    long long mtiles;
+    tile_geometry(B, Hs, Ws, lbm, wt, ht, nt, mtiles);
+    if (mtiles * (Co / lbn) * nphase < kLargeMinTiles) return;
+    bm = lbm;
+    bn = lbn;
 }
 
 // T2 corner pixel (2*Hi, 2*Wi): only tap (2,2) on input pixel (Hi-1, Wi-1) reaches it.  One warp per (b, o), staged
@@ -363,34 +415,39 @@ void site_grid(int Hi, int Wi, int Ho, int Wo, int mode, int& Hs, int& Ws) {
     if (mode == 2) { Hs = Hi; Ws = Wi; } else { Hs = Ho; Ws = Wo; }
 }
 
-template <int BLOCK_N, bool X3>
+template <int BM, int BN, bool X3>
 int launch(const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorMap& mb, const CUtensorMap& mb2, float* y,
            const TcParams& p, int mtiles, cudaStream_t st) {
-    using L = SmemLayout<BLOCK_N>;
+    using L = TileCfg<BM, BN>;
     static bool attr_set = false;   // per-process, idempotent
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
+        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BM, BN, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
         if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "cudaFuncSetAttribute(conv_tc_kernel)", cudaGetErrorString(e));
         attr_set = true;
     }
-    const long long total = static_cast<long long>(mtiles) * (p.Co / BLOCK_N) * p.nphase * p.ksplit;
+    const long long total = static_cast<long long>(mtiles) * (p.Co / BN) * p.nphase * p.ksplit;
     if (total > 2147483647LL) return fail(GIFB200_E_SHAPE, "conv2d_tc: too many tiles");
-    const int grid = total < 2 * kNumSMs ? static_cast<int>(total) : 2 * kNumSMs;   // persistent: <= 2 CTAs per SM
-    conv_tc_kernel<BLOCK_N, X3><<<grid, kTcThreads, L::kDynamic, st>>>(ma, ma2, mb, mb2, y, p, mtiles, static_cast<int>(total));
+    constexpr int kMaxGrid = L::kMinBlocks * kNumSMs;     // persistent: kMinBlocks CTAs per SM
+    const int grid = total < kMaxGrid ? static_cast<int>(total) : kMaxGrid;
+    conv_tc_kernel<BM, BN, X3><<<grid, L::kThreads, L::kDynamic, st>>>(ma, ma2, mb, mb2, y, p, mtiles, static_cast<int>(total));
     GIFB200_LAUNCH_CHECK("conv_tc_kernel");
     return GIFB200_OK;
 }
 
-int launch_any(int bn, bool x3, const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorMap& mb, const CUtensorMap& mb2,
-               float* y, const TcParams& p, int mtiles, cudaStream_t st) {
-    if (x3) {
-        if (bn == 128) return launch<128, true>(ma, ma2, mb, mb2, y, p, mtiles, st);
-        if (bn == 64) return launch<64, true>(ma, ma2, mb, mb2, y, p, mtiles, st);
-        return launch<32, true>(ma, ma2, mb, mb2, y, p, mtiles, st);
-    }
-    if (bn == 128) return launch<128, false>(ma, ma2, mb, mb2, y, p, mtiles, st);
-    if (bn == 64) return launch<64, false>(ma, ma2, mb, mb2, y, p, mtiles, st);
-    return launch<32, false>(ma, ma2, mb, mb2, y, p, mtiles, st);
+template <bool X3>
+int launch_tile(int bm, int bn, const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorMap& mb, const CUtensorMap& mb2,
+                float* y, const TcParams& p, int mtiles, cudaStream_t st) {
+    if (bm == 256) return launch<256, 128, X3>(ma, ma2, mb, mb2, y, p, mtiles, st);
+    if (bn == 256) return launch<128, 256, X3>(ma, ma2, mb, mb2, y, p, mtiles, st);
+    if (bn == 128) return launch<128, 128, X3>(ma, ma2, mb, mb2, y, p, mtiles, st);
+    if (bn == 64) return launch<128, 64, X3>(ma, ma2, mb, mb2, y, p, mtiles, st);
+    return launch<128, 32, X3>(ma, ma2, mb, mb2, y, p, mtiles, st);
+}
+
+int launch_any(int bm, int bn, bool x3, const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorMap& mb,
+               const CUtensorMap& mb2, float* y, const TcParams& p, int mtiles, cudaStream_t st) {
+    return x3 ? launch_tile<true>(bm, bn, ma, ma2, mb, mb2, y, p, mtiles, st)
+              : launch_tile<false>(bm, bn, ma, ma2, mb, mb2, y, p, mtiles, st);
 }
 
 }  // namespace
@@ -416,7 +473,7 @@ static int ksplit_of(int B, int Hi, int Wi, int Ci, int Ho, int Wo, int Co, int 
     int Hs, Ws, wt, ht, nt;
     long long mtiles;
     site_grid(Hi, Wi, Ho, Wo, mode, Hs, Ws);
-    tile_geometry(B, Hs, Ws, wt, ht, nt, mtiles);
+    tile_geometry(B, Hs, Ws, 128, wt, ht, nt, mtiles);
     const int bn = pick_block_n(Co);
     if (bn == 0) return 1;
     return pick_ksplit(mtiles * (Co / bn), k * k * (Ci / kBlockK), mode);
@@ -460,11 +517,13 @@ int conv2d_tc(const float* x, const float* w, float* y, int B, int Hi, int Wi, i
     memset(&p, 0, sizeof(p));
     p.B = B; p.Ci = Ci; p.Co = Co; p.Ho = Ho; p.Wo = Wo; p.epi = epi;
     site_grid(Hi, Wi, Ho, Wo, mode, p.Hs, p.Ws);
+    p.ksplit = ksplit_of(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode);
+    int bm, bn;
+    pick_tile(B, p.Hs, p.Ws, Co, mode == 2 ? 4 : 1, p.ksplit, bm, bn);
     long long mtiles;
-    tile_geometry(B, p.Hs, p.Ws, p.wt, p.ht, p.nt, mtiles);
+    tile_geometry(B, p.Hs, p.Ws, bm, p.wt, p.ht, p.nt, mtiles);
     p.tiles_x = p.Ws / p.wt; p.tiles_y = p.Hs / p.ht;
     GIFB200_REQUIRE(mtiles <= 2147483647LL, GIFB200_E_SHAPE, "conv2d_tc: too many tiles");
-    p.ksplit = ksplit_of(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode);
     if (p.ksplit > 1) {
         p.part_stride = static_cast<long long>(B) * Ho * Wo * Co;
         p.part = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(reinterpret_cast<char*>(wst) + staged_weight_bytes(Ci, Co, k) - 256) + 255) &
@@ -526,17 +585,20 @@ int conv2d_tc(const float* x, const float* w, float* y, int B, int Hi, int Wi, i
         if (rc == GIFB200_OK && x3) rc = encode_map(&ma2, xb + x_plane * es, 5, dims, strides, box, swz, dt, estr);
     }
     if (rc != GIFB200_OK) return rc;
-    const int bn = pick_block_n(Co);
-    {
+    // weight maps (hi, lo) with a box of box_n output channels: the B tile of one stage
+    auto encode_b = [&](int box_n, CUtensorMap& m, CUtensorMap& m2) {
         const cuuint64_t dims[3] = {static_cast<cuuint64_t>(Ci), static_cast<cuuint64_t>(Co), static_cast<cuuint64_t>(T)};
         const cuuint64_t strides[2] = {static_cast<cuuint64_t>(Ci) * es, static_cast<cuuint64_t>(Co) * Ci * es};
-        const cuuint32_t box[3] = {kBlockK, static_cast<cuuint32_t>(bn), 1};
-        rc = encode_map(&mb, wb, 3, dims, strides, box, swz, dt);
-        if (rc == GIFB200_OK && x3) rc = encode_map(&mb2, wb + w_plane * es, 3, dims, strides, box, swz, dt);
-        if (rc != GIFB200_OK) return rc;
-    }
-    if (!x3) { ma2 = ma; mb2 = mb; }
-    rc = launch_any(bn, x3, ma, ma2, mb, mb2, y, p, static_cast<int>(mtiles), st);
+        const cuuint32_t box[3] = {kBlockK, static_cast<cuuint32_t>(box_n), 1};
+        int r = encode_map(&m, wb, 3, dims, strides, box, swz, dt);
+        if (r == GIFB200_OK && x3) r = encode_map(&m2, wb + w_plane * es, 3, dims, strides, box, swz, dt);
+        if (!x3) m2 = m;
+        return r;
+    };
+    rc = encode_b(bn, mb, mb2);
+    if (rc != GIFB200_OK) return rc;
+    if (!x3) ma2 = ma;
+    rc = launch_any(bm, bn, x3, ma, ma2, mb, mb2, y, p, static_cast<int>(mtiles), st);
     if (rc == GIFB200_OK && p.ksplit > 1) {
         const long long n4 = p.part_stride / 4;
         int blocks = cdiv(n4, 256);
@@ -548,7 +610,11 @@ int conv2d_tc(const float* x, const float* w, float* y, int B, int Hi, int Wi, i
     // ---- T2 border: output row Y = 2*Hi and column X = 2*Wi (the sites y = Hi / x = Wi that the power-of-two site grid does
     // not cover).  Row Y = 2*Hi only sees kernel row kh = 2 applied to input row Hi-1: a 1-D transposed convolution along x;
     // likewise the column along y with kw = 2.  Both run through the SAME tensor-core kernel on 1-row / 1-column views of
-    // the input (two more launches of ~1/64 of the main work each); the single corner pixel is a dot product per (b, o).
+    // the input (two more launches of ~1/64 of the main work each, always with 128 x BN tiles); the single corner pixel is
+    // a dot product per (b, o).
+    const int bn_e = pick_block_n(Co);
+    CUtensorMap mbe = mb, mbe2 = mb2;
+    if (bn_e != bn) rc = encode_b(bn_e, mbe, mbe2);
     for (int edge = 0; edge < 2 && rc == GIFB200_OK; ++edge) {
         const bool row = edge == 0;
         TcParams q;
@@ -584,7 +650,7 @@ int conv2d_tc(const float* x, const float* w, float* y, int B, int Hi, int Wi, i
         if (rc == GIFB200_OK && x3) rc = encode_map(&me2, base + x_plane * es, 4, dims, strides, box, swz, dt);
         if (rc != GIFB200_OK) return rc;
         if (!x3) me2 = me;
-        rc = launch_any(bn, x3, me, me2, mb, mb2, y, q, static_cast<int>(mt_e), st);
+        rc = launch_any(128, bn_e, x3, me, me2, mbe, mbe2, y, q, static_cast<int>(mt_e), st);
     }
     if (rc != GIFB200_OK) return rc;
     {

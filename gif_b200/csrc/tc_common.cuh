@@ -62,6 +62,11 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// warpgroup register reallocation: every thread of the warpgroup executes it; R is a multiple of 8 in [24, 256]
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void fence_regs(float* d) {
@@ -86,6 +91,11 @@ __device__ __forceinline__ void wgmma_bf16(float* d, uint64_t da, uint64_t db, i
 #define GIF_R32 GIF_R16 ", " GIF_R8(16, 17, 18, 19, 20, 21, 22, 23) ", " GIF_R8(24, 25, 26, 27, 28, 29, 30, 31)
 #define GIF_R64 GIF_R32 ", " GIF_R8(32, 33, 34, 35, 36, 37, 38, 39) ", " GIF_R8(40, 41, 42, 43, 44, 45, 46, 47) ", " \
     GIF_R8(48, 49, 50, 51, 52, 53, 54, 55) ", " GIF_R8(56, 57, 58, 59, 60, 61, 62, 63)
+#define GIF_F128 GIF_F64, GIF_F8(64), GIF_F8(72), GIF_F8(80), GIF_F8(88), GIF_F8(96), GIF_F8(104), GIF_F8(112), GIF_F8(120)
+#define GIF_R128 GIF_R64 ", " GIF_R8(64, 65, 66, 67, 68, 69, 70, 71) ", " GIF_R8(72, 73, 74, 75, 76, 77, 78, 79) ", " \
+    GIF_R8(80, 81, 82, 83, 84, 85, 86, 87) ", " GIF_R8(88, 89, 90, 91, 92, 93, 94, 95) ", " \
+    GIF_R8(96, 97, 98, 99, 100, 101, 102, 103) ", " GIF_R8(104, 105, 106, 107, 108, 109, 110, 111) ", " \
+    GIF_R8(112, 113, 114, 115, 116, 117, 118, 119) ", " GIF_R8(120, 121, 122, 123, 124, 125, 126, 127)
 // operands after the accumulators: descriptors %R, %R+1, scale-d %R+2 (, transpose immediates %R+3, %R+4)
 #define GIF_WGMMA_TF32(N, R, S0, S1, S2) \
     template <> \
@@ -108,9 +118,11 @@ __device__ __forceinline__ void wgmma_bf16(float* d, uint64_t da, uint64_t db, i
 GIF_WGMMA_TF32(32, 16, 16, 17, 18)
 GIF_WGMMA_TF32(64, 32, 32, 33, 34)
 GIF_WGMMA_TF32(128, 64, 64, 65, 66)
+GIF_WGMMA_TF32(256, 128, 128, 129, 130)
 GIF_WGMMA_BF16(32, 16, 16, 17, 18, 19, 20, 0)
 GIF_WGMMA_BF16(64, 32, 32, 33, 34, 35, 36, 0)
 GIF_WGMMA_BF16(128, 64, 64, 65, 66, 67, 68, 0)
+GIF_WGMMA_BF16(256, 128, 128, 129, 130, 131, 132, 0)
 GIF_WGMMA_BF16(32, 16, 16, 17, 18, 19, 20, 1)
 GIF_WGMMA_BF16(64, 32, 32, 33, 34, 35, 36, 1)
 
