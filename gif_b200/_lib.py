@@ -49,6 +49,7 @@ SIGNATURES = {
     "gifb200_torgb_bwd_w": (_i, [_p, _p, _p, _i, _i, _i, _p]),
     "gifb200_sgemm": (_i, [_i, _i, _i, _i, _i, _f, _p, _i, _p, _i, _p, _i, _p]),
     "gifb200_cond_down": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _p]),
+    "gifb200_cond_up": (_i, [_p, _p, _i, _i, _i, _i, _i, _i, _p]),
     "gifb200_rasterize_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "gifb200_rasterize_fwd": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _sz, _p]),
     "gifb200_rasterize_fwd_ex": (_i, [_p] * 7 + [_i] * 5 + [_p, _sz, _p]),

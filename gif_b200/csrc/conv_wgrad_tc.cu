@@ -17,6 +17,12 @@
 // the 4th chunk is a duplicate) -- chunk kh then accumulates kernel row kh, the KW shifted Bg tiles give the kernel
 // columns, and ONE CTA produces all 9 taps (no kh split).
 //
+// NARROW variant (AC = 2: Cs == 64, or Cs == 32 with Cb <= 64 for the 1x1 stride-1 layers -- the 512^2 / 1024^2 layers): M = 64, two A
+// chunks.  tf32: the 8 mma.sync warps are 2 (rows) x 4 (columns).  X3: both warpgroups issue m64 wgmma on all 64 rows,
+// warpgroup wg on the 16-pixel slice wg of every stage; at the end warpgroup 1 hands its sums to warpgroup 0 through the
+// drained stage ring (fixed order: slice 0 + slice 1).  With Cs == 32 the second chunk repeats the first and its rows are
+// not written.
+//
 // X3 = true ("bf16x3", gifb200_conv2d_wgrad impl 3): both operands arrive as two bf16 planes (hi, lo; gifb200_split_bf16).
 // 16-bit MN-major tiles of 32 channels use the canonical SWIZZLE_64B layout (rows of 64 bytes, 8-pixel K atoms of 512 B; TMA
 // side CU_TENSOR_MAP_SWIZZLE_64B), which wgmma reads transposed; a stage holds the hi and the lo chunk set of each operand --
@@ -31,7 +37,6 @@ namespace {
 
 constexpr int kWgStages = 4;
 constexpr int kPix = 32;                       // pixels (GEMM K) per stage
-constexpr int kAChunks = 4;                    // M = 128 small channels
 constexpr int kWgConsumerWarps = 8;            // two warpgroups (X3: wgmma on rows 0-63 / 64-127) or 4 x 2 mma.sync warps
 constexpr int kWgThreads = 32 * kWgConsumerWarps + 32;   // + one TMA producer warp
 
@@ -51,14 +56,14 @@ constexpr int kHaloRows = kPix + 2;                 // 34 pixel rows: the 32 of 
 
 // HALO (fp32, stride-1 layers with Ws >= 32): the KW shifted big-tensor tiles of a stage overlap in all but 2 pixel rows, so
 // the stage holds ONE (32 + 2)-row tile per 32-channel chunk and tap kw reads it from pixel row kw on.
-template <int KW, int BLOCK_N, bool HALO = false, bool X3 = false>
+template <int KW, int BLOCK_N, bool HALO = false, bool X3 = false, int AC = 4>
 struct WgSmem {
     static constexpr int kRowBytes = X3 ? 64 : 128;                   // 32 channels of one pixel
     static constexpr int kChunkBytes = kPix * kRowBytes;              // one 32-channel x 32-pixel chunk: 4 KB fp32, 2 KB bf16
     static constexpr int kHaloChunkBytes = 5120;                      // 34 rows of 128 B padded to the 1024 B swizzle atom
     static constexpr int kPlanes = X3 ? 2 : 1;                        // hi and lo chunk sets, hi first
     static constexpr int kBChunks = BLOCK_N / 32;
-    static constexpr int kAPlaneBytes = kAChunks * kChunkBytes;
+    static constexpr int kAPlaneBytes = AC * kChunkBytes;         // AC 32-channel A chunks: M = 32 * AC small channels
     static constexpr int kABytes = kPlanes * kAPlaneBytes;
     static constexpr int kBPlaneBytes = kBChunks * (HALO ? kHaloChunkBytes : kChunkBytes);   // one tap (or the halo tile), one plane
     static constexpr int kBBytesPerTap = kPlanes * kBPlaneBytes;
@@ -76,13 +81,14 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int ch) {
     return static_cast<uint32_t>(row * 128 + ((((ch >> 2) ^ row) & 7) << 4) + (ch & 3) * 4);
 }
 
-template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3>
+template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_s,
                                                                  const __grid_constant__ CUtensorMap map_s2,
                                                                  const __grid_constant__ CUtensorMap map_b,
                                                                  const __grid_constant__ CUtensorMap map_b2,
                                                                  float* __restrict__ part, const WgParams p) {
-    using L = WgSmem<KW, BLOCK_N, HALO, X3>;
+    using L = WgSmem<KW, BLOCK_N, HALO, X3, AC>;
+    constexpr int kM = 32 * AC;
     constexpr int kChunkBytes = L::kChunkBytes;
     constexpr int kHaloChunkBytes = L::kHaloChunkBytes;
     constexpr int kNStages = L::kStages;
@@ -92,7 +98,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     uint64_t* empty_bar = full_bar + kNStages;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    const int ms = blockIdx.x;                       // 128-channel tile of the small tensor
+    const int ms = blockIdx.x;                       // kM-channel tile of the small tensor
     const int nb = blockIdx.y;                       // BLOCK_N-channel tile of the big tensor
     const int kh = STACK ? 0 : blockIdx.z / p.splits, split = STACK ? blockIdx.z : blockIdx.z % p.splits;
     const long long per = (p.units + p.splits - 1) / p.splits;
@@ -139,10 +145,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
                         const CUtensorMap* mb_ = pl ? &map_b2 : &map_b;
                         uint8_t* a_pl = a_dst + pl * L::kAPlaneBytes;
                         if (r == 0 || !p.mr_s) {
-                            for (int c = 0; c < kAChunks; ++c) {
+                            for (int c = 0; c < AC; ++c) {
                                 if (STACK)   // chunk kh = S shifted by dy = 1 - kh rows (rows outside the image are zero-filled)
                                     tma_load_4d(a_pl + c * kChunkBytes + r * row_bytes, ms_, &full_bar[stage], 0, x0,
                                                 y + 1 - (c < 3 ? c : 2), n);
+                                else if (AC == 2)   // Cs == 32: the second chunk repeats the first
+                                    tma_load_4d(a_pl + c * kChunkBytes + r * row_bytes, ms_, &full_bar[stage],
+                                                c * 32 < p.Cs ? c * 32 : 0, x0, y, n);
                                 else
                                     tma_load_4d(a_pl + c * kChunkBytes + r * row_bytes, ms_, &full_bar[stage], ms * 128 + c * 32, x0, y, n);
                             }
@@ -180,8 +189,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
     const int g = lane >> 2, tq = lane & 3;
     if (X3) {
         // wgmma, both operands MN-major SWIZZLE_64B (rows of 64 B = 32 bf16, 8-pixel K atoms of 512 B): LBO = distance between
-        // 32-channel chunks, SBO = 512 B.  Warpgroup wg owns A chunks 2wg, 2wg+1 (its 64 rows); one accumulator per tap.
+        // 32-channel chunks, SBO = 512 B.  AC = 4: warpgroup wg owns A chunks 2wg, 2wg+1 (its 64 rows) and both 16-pixel
+        // slices; AC = 2: all 64 rows and slice wg.  One accumulator per tap.
         const int wg = warp >> 2, wq = warp & 3;
+        constexpr int kSlices = AC == 4 ? kPix / 16 : 1;
         constexpr int kAcc = BLOCK_N / 2;
         float acc[KW][kAcc];
 #pragma unroll
@@ -193,8 +204,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
         for (int it = 0; it < iters; ++it) {
             mbar_wait(&full_bar[stage], ph);
             const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-            const uint64_t adesc = make_smem_desc(a_addr + wg * 2 * kChunkBytes, kChunkBytes, 512, 2);
-            const uint64_t adesc_lo = make_smem_desc(a_addr + L::kAPlaneBytes + wg * 2 * kChunkBytes, kChunkBytes, 512, 2);
+            const uint32_t a_row = AC == 4 ? wg * 2 * kChunkBytes : 0;
+            const uint64_t adesc = make_smem_desc(a_addr + a_row, kChunkBytes, 512, 2);
+            const uint64_t adesc_lo = make_smem_desc(a_addr + L::kAPlaneBytes + a_row, kChunkBytes, 512, 2);
             wgmma_fence();
 #pragma unroll
             for (int kw = 0; kw < KW; ++kw) {
@@ -203,7 +215,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
                 const uint64_t bdesc = make_smem_desc(b_addr, kChunkBytes, 512, 2);
                 const uint64_t bdesc_lo = make_smem_desc(b_addr + L::kBPlaneBytes, kChunkBytes, 512, 2);
 #pragma unroll
-                for (int j = 0; j < kPix / 16; ++j) {   // 16 pixels per MMA = two 8-pixel atoms: next slice = +1024 B (>>4 = 64)
+                for (int jj = 0; jj < kSlices; ++jj) {   // 16 pixels per MMA = two 8-pixel atoms: next slice = +1024 B (>>4 = 64)
+                    const int j = AC == 4 ? jj : wg;
                     wgmma_bf16<BLOCK_N>(acc[kw], adesc_lo + 64 * j, bdesc + 64 * j, 1, Trans<1>());
                     wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc_lo + 64 * j, 1, Trans<1>());
                     wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc + 64 * j, 1, Trans<1>());
@@ -220,12 +233,31 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
         wgmma_wait<0>();
 #pragma unroll
         for (int kw = 0; kw < KW; ++kw) fence_regs<kAcc>(acc[kw]);
+        if constexpr (AC == 2) {
+            // every MMA of both warpgroups has completed past the barrier, so the stage ring is free to carry the exchange
+            static_assert(KW * kAcc * 128 * 4 <= kNStages * L::kStageBytes, "exchange buffer exceeds the stage ring");
+            float* xch = reinterpret_cast<float*>(smem) + (threadIdx.x & 127);
+            asm volatile("bar.sync 1, %0;" ::"n"(32 * kWgConsumerWarps) : "memory");
+            if (wg == 1) {
+#pragma unroll
+                for (int kw = 0; kw < KW; ++kw)
+#pragma unroll
+                    for (int i = 0; i < kAcc; ++i) xch[(kw * kAcc + i) * 128] = acc[kw][i];
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(32 * kWgConsumerWarps) : "memory");
+            if (wg == 1) return;
+#pragma unroll
+            for (int kw = 0; kw < KW; ++kw)
+#pragma unroll
+                for (int i = 0; i < kAcc; ++i) acc[kw][i] += xch[(kw * kAcc + i) * 128];
+        }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            const int r = wg * 64 + wq * 16 + g + 8 * h;      // row of the 128-row A tile
+            const int r = (AC == 4 ? wg * 64 : 0) + wq * 16 + g + 8 * h;      // row of the kM-row A tile
             const int q = r >> 5;
             if (STACK && q == 3) continue;                    // duplicate chunk
-            const int cs = STACK ? (r & 31) : ms * 128 + r;
+            if (AC == 2 && r >= p.Cs) continue;               // Cs == 32: repeated chunk
+            const int cs = STACK ? (r & 31) : ms * kM + r;
 #pragma unroll
             for (int kw = 0; kw < KW; ++kw) {
                 const int t = (STACK ? q : kh) * p.k + kw;
@@ -236,10 +268,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
             }
         }
     } else {
-        // mma.sync m16n8k8 tf32: warp (wm, wn) computes rows 32wm..32wm+31 (= A chunk wm) x columns wn*BLOCK_N/2 .. of every
-        // tap.  Fragments are gathered from the SWIZZLE_128B tiles with 32-bit shared loads.
-        const int wm = warp & 3, wn = warp >> 2;
-        constexpr int NT = BLOCK_N / 16;                 // n8 tiles per warp
+        // mma.sync m16n8k8 tf32: warp (wm, wn) computes rows 32wm..32wm+31 (= A chunk wm) x columns wn*BLOCK_N/kWN .. of
+        // every tap.  Fragments are gathered from the SWIZZLE_128B tiles with 32-bit shared loads.
+        constexpr int kWN = kWgConsumerWarps / AC;       // warps along N: 2 (AC = 4) or 4 (AC = 2)
+        const int wm = warp % AC, wn = warp / AC;
+        constexpr int NT = BLOCK_N / (8 * kWN);          // n8 tiles per warp
         float acc[KW][2][NT][4];
 #pragma unroll
         for (int kw = 0; kw < KW; ++kw)
@@ -271,7 +304,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
                 for (int kw = 0; kw < KW; ++kw) {
 #pragma unroll
                     for (int nt = 0; nt < NT; ++nt) {
-                        const int n = wn * (BLOCK_N / 2) + nt * 8 + g;
+                        const int n = wn * (BLOCK_N / kWN) + nt * 8 + g;
                         const uint8_t* chunk = HALO ? sb + (n >> 5) * kHaloChunkBytes : sb + kw * L::kBBytesPerTap + (n >> 5) * kChunkBytes;
                         const int row = HALO ? k0 + kw : k0;     // HALO: tap kw starts kw pixel rows into the halo tile
                         uint32_t b[2];
@@ -287,16 +320,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
             if (++stage == kNStages) { stage = 0; ph ^= 1; }
         }
         if (STACK && wm == 3) return;                           // duplicate chunk
+        if (AC == 2 && wm * 32 >= p.Cs) return;                 // Cs == 32: repeated chunk
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = wm * 32 + mt * 16 + g + 8 * h;
-                const int cs = STACK ? (r & 31) : ms * 128 + r;
+                const int cs = STACK ? (r & 31) : ms * kM + r;
 #pragma unroll
                 for (int kw = 0; kw < KW; ++kw) {
                     const int t = (STACK ? wm : kh) * p.k + kw;
-                    float* obase = pbase + (static_cast<long long>(t) * p.Cs + cs) * p.Cb + nb * BLOCK_N + wn * (BLOCK_N / 2) + 2 * tq;
+                    float* obase = pbase + (static_cast<long long>(t) * p.Cs + cs) * p.Cb + nb * BLOCK_N + wn * (BLOCK_N / kWN) + 2 * tq;
 #pragma unroll
                     for (int nt = 0; nt < NT; ++nt)
                         *reinterpret_cast<float2*>(obase + nt * 8) = make_float2(acc[kw][mt][nt][2 * h], acc[kw][mt][nt][2 * h + 1]);
@@ -332,17 +366,17 @@ int pick_bn(int Cb) {
 
 struct WgMaps { CUtensorMap s, s2, b, b2; };
 
-template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3>
+template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC>
 int launch_wg(const WgMaps& m, float* out, float* part, const WgParams& p, cudaStream_t st) {
-    using L = WgSmem<KW, BLOCK_N, HALO, X3>;
+    using L = WgSmem<KW, BLOCK_N, HALO, X3, AC>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
+        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
         if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "cudaFuncSetAttribute(wgrad_tc_kernel)", cudaGetErrorString(e));
         attr_set = true;
     }
-    dim3 grid(STACK ? 1 : p.Cs / 128, p.Cb / BLOCK_N, STACK ? p.splits : p.k * p.splits);
-    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
+    dim3 grid(STACK || AC == 2 ? 1 : p.Cs / 128, p.Cb / BLOCK_N, STACK ? p.splits : p.k * p.splits);
+    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
     GIFB200_LAUNCH_CHECK("wgrad_tc_kernel");
     const int T = p.k * p.k;
     const long long total = static_cast<long long>(T) * p.Cs * p.Cb;
@@ -352,6 +386,11 @@ int launch_wg(const WgMaps& m, float* out, float* part, const WgParams& p, cudaS
     GIFB200_LAUNCH_CHECK("wgrad_reduce_kernel");
     return GIFB200_OK;
 }
+
+inline bool is_stack(int Cs, int k, int mode) { return Cs == 32 && mode == 0 && k == 3; }
+// 32 small channels only up to 64 big ones: with 128 (the 1x1 256^2 discriminator stem's R1 term, Cs = 9 padded to 32) the
+// exact SIMT kernel keeps the 256^2 step's results bitwise as they were
+inline bool is_narrow(int Cs, int Cb, int k, int mode) { return Cs == 64 || (Cs == 32 && mode == 0 && k == 1 && Cb <= 64); }
 
 void roles(int Hi, int Wi, int Ci, int Ho, int Wo, int Co, int mode, int& Hs, int& Ws, int& Cs, int& Hb, int& Wb, int& Cb) {
     if (mode == 2) { Hs = Hi; Ws = Wi; Cs = Ci; Hb = Ho; Wb = Wo; Cb = Co; }
@@ -367,8 +406,7 @@ bool conv2d_wgrad_tc_supported(int B, int Hi, int Wi, int Ci, int Ho, int Wo, in
     if (mode == 2 && !(Ho == 2 * Hi + 1 && Wo == 2 * Wi + 1)) return false;
     int Hs, Ws, Cs, Hb, Wb, Cb;
     roles(Hi, Wi, Ci, Ho, Wo, Co, mode, Hs, Ws, Cs, Hb, Wb, Cb);
-    const bool stack = (Cs == 32 && mode == 0 && k == 3);
-    if ((Cs % 128 != 0 && !stack) || pick_bn(Cb) == 0) return false;
+    if ((Cs % 128 != 0 && !is_stack(Cs, k, mode) && !is_narrow(Cs, Cb, k, mode)) || pick_bn(Cb) == 0) return false;
     if (!pow2i(Hs) || !pow2i(Ws) || Ws < 4 || Hs < 4) return false;
     if ((static_cast<long long>(B) * Hs * Ws) % kPix != 0) return false;
     const int pw = Ws < kPix ? Ws : kPix;
@@ -381,9 +419,9 @@ static long long wgrad_splits(int B, int Hi, int Wi, int Ci, int Ho, int Wo, int
     roles(Hi, Wi, Ci, Ho, Wo, Co, mode, Hs, Ws, Cs, Hb, Wb, Cb);
     const long long units = static_cast<long long>(B) * Hs * Ws / kPix;
     const int bn = pick_bn(Cb);
-    const bool stack = (Cs == 32 && mode == 0 && k == 3);
-    const long long base_ctas = stack ? (Cb / bn) : static_cast<long long>(Cs / 128) * (Cb / bn) * k;
-    // ONE wave: the kernel runs one CTA per SM (130-160 KB of shared memory), so the grid must not exceed the SM count
+    const long long m_tiles = is_narrow(Cs, Cb, k, mode) ? 1 : Cs / 128;
+    const long long base_ctas = is_stack(Cs, k, mode) ? (Cb / bn) : m_tiles * (Cb / bn) * k;
+    // ONE wave: the kernel runs one CTA per SM (90-160 KB of shared memory), so the grid must not exceed the SM count
     // (rounding the split count up would leave a second wave of a few stragglers that doubles the kernel time).
     long long splits = kNumSMs / base_ctas;
     if (splits > units) splits = units;
@@ -398,8 +436,16 @@ size_t conv2d_wgrad_tc_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, in
 }
 
 template <bool X3>
-static int dispatch_wg(int k, int bn, bool stack, bool halo, const WgMaps& m, float* gw, float* part, const WgParams& p, cudaStream_t st) {
-#define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3>(m, gw, part, p, st)
+static int dispatch_wg(int k, int bn, bool stack, bool narrow, bool halo, const WgMaps& m, float* gw, float* part, const WgParams& p,
+                       cudaStream_t st) {
+#define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3, 4>(m, gw, part, p, st)
+#define GIFB200_WGN(KW, BN, HA) launch_wg<KW, BN, false, HA, X3, 2>(m, gw, part, p, st)
+    if (narrow) {
+        if constexpr (!X3)
+            if (halo) return bn == 64 ? GIFB200_WGN(3, 64, true) : GIFB200_WGN(3, 32, true);
+        if (k == 3) return bn == 64 ? GIFB200_WGN(3, 64, false) : GIFB200_WGN(3, 32, false);
+        return bn == 64 ? GIFB200_WGN(1, 64, false) : GIFB200_WGN(1, 32, false);
+    }
     if constexpr (!X3) {
         if (stack && halo) return bn == 64 ? GIFB200_WG(3, 64, true, true) : GIFB200_WG(3, 32, true, true);
         if (halo) return bn == 64 ? GIFB200_WG(3, 64, false, true) : GIFB200_WG(3, 32, false, true);
@@ -407,6 +453,7 @@ static int dispatch_wg(int k, int bn, bool stack, bool halo, const WgMaps& m, fl
     if (stack) return bn == 64 ? GIFB200_WG(3, 64, true, false) : GIFB200_WG(3, 32, true, false);
     if (k == 3) return bn == 64 ? GIFB200_WG(3, 64, false, false) : GIFB200_WG(3, 32, false, false);
     return bn == 64 ? GIFB200_WG(1, 64, false, false) : GIFB200_WG(1, 32, false, false);
+#undef GIFB200_WGN
 #undef GIFB200_WG
 }
 
@@ -434,7 +481,7 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
     p.stride_cb = mode == 2 ? stride_o : stride_i;
     p.stride_t = static_cast<long long>(Co) * Ci;
     const int bn = pick_bn(p.Cb);
-    const bool stack = (p.Cs == 32 && mode == 0 && k == 3);
+    const bool stack = is_stack(p.Cs, k, mode), narrow = is_narrow(p.Cs, p.Cb, k, mode);
     p.splits = static_cast<int>(wgrad_splits(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, nullptr));
     p.part_stride = static_cast<long long>(k) * k * Co * Ci;
     // operand element size / tile layout: fp32 (SWIZZLE_128B, read by mma.sync fragments) or bf16 planes (MN-major SWIZZLE_64B)
@@ -490,7 +537,8 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
         if (rc != GIFB200_OK) return rc;
     }
     if (!x3) { m.s2 = m.s; m.b2 = m.b; }
-    return x3 ? dispatch_wg<true>(k, bn, stack, halo, m, gw, part, p, st) : dispatch_wg<false>(k, bn, stack, halo, m, gw, part, p, st);
+    return x3 ? dispatch_wg<true>(k, bn, stack, narrow, halo, m, gw, part, p, st)
+              : dispatch_wg<false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
 }
 
 }  // namespace gifb200

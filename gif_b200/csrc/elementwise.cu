@@ -747,6 +747,77 @@ __global__ void __launch_bounds__(256) cond_down_adj_kernel(float* __restrict__ 
     }
 }
 
+// Bilinear upsampling by a power of two s (F.interpolate, align_corners=False): output index o reads source coordinate
+// max((o + 0.5) / s - 0.5, 0) -- exact in fp32 -- between i0 = floor and i1 = min(i0 + 1, n - 1), weight l1 on i1.
+__device__ __forceinline__ void up_taps(int o, int s, int n, int& i0, int& i1, float& l1) {
+    const float src = fmaxf((o + 0.5f) / s - 0.5f, 0.f);
+    i0 = static_cast<int>(src);
+    i1 = i0 < n - 1 ? i0 + 1 : i0;
+    l1 = src - i0;
+}
+
+// weight of source index i in output index o (both taps land on i at the clamped edge)
+__device__ __forceinline__ float up_weight(int o, int i, int s, int n) {
+    int i0, i1;
+    float l1;
+    up_taps(o, s, n, i0, i1, l1);
+    return (i0 == i ? 1.f - l1 : 0.f) + (i1 == i ? l1 : 0.f);
+}
+
+// y (B, sH, sW, C) = bilinear upsampling of x (B, H, W, C)
+__global__ void __launch_bounds__(256) cond_up_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
+                                                      int C, int s) {
+    const int Ho = H * s, Wo = W * s;
+    const long long total = static_cast<long long>(B) * Ho * Wo * C;
+    for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
+         e += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int c = static_cast<int>(e % C);
+        long long r = e / C;
+        const int xo = static_cast<int>(r % Wo); r /= Wo;
+        const int yo = static_cast<int>(r % Ho);
+        const int b = static_cast<int>(r / Ho);
+        int y0, y1, x0, x1;
+        float ly, lx;
+        up_taps(yo, s, H, y0, y1, ly);
+        up_taps(xo, s, W, x0, x1, lx);
+        const float* base = x + static_cast<long long>(b) * H * W * C + c;
+        const float top = (1.f - lx) * base[(static_cast<long long>(y0) * W + x0) * C] + lx * base[(static_cast<long long>(y0) * W + x1) * C];
+        const float bot = (1.f - lx) * base[(static_cast<long long>(y1) * W + x0) * C] + lx * base[(static_cast<long long>(y1) * W + x1) * C];
+        y[e] = (1.f - ly) * top + ly * bot;
+    }
+}
+
+// adjoint, as a gather (no atomics): gx[b, i, j] = sum over the outputs (o, q) that read (i, j) of wy * wx * gy[b, o, q].
+// Output o reads source rows floor(src) and floor(src) + 1, so only o in [s(i - 1), s(i + 2)) can read row i.
+__global__ void __launch_bounds__(256) cond_up_adj_kernel(float* __restrict__ gx, const float* __restrict__ gy, int B, int H,
+                                                          int W, int C, int s) {
+    const int Ho = H * s, Wo = W * s;
+    const long long total = static_cast<long long>(B) * H * W * C;
+    for (long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total;
+         e += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int c = static_cast<int>(e % C);
+        long long r = e / C;
+        const int j = static_cast<int>(r % W); r /= W;
+        const int i = static_cast<int>(r % H);
+        const int b = static_cast<int>(r / H);
+        const int o0 = max(s * (i - 1), 0), o1 = min(s * (i + 2), Ho);
+        const int q0 = max(s * (j - 1), 0), q1 = min(s * (j + 2), Wo);
+        const float* g = gy + static_cast<long long>(b) * Ho * Wo * C + c;
+        float acc = 0.f;
+        for (int o = o0; o < o1; ++o) {
+            const float wy = up_weight(o, i, s, H);
+            if (wy == 0.f) continue;
+            float row = 0.f;
+            for (int q = q0; q < q1; ++q) {
+                const float wx = up_weight(q, j, s, W);
+                if (wx != 0.f) row += wx * g[(static_cast<long long>(o) * Wo + q) * C];
+            }
+            acc += wy * row;
+        }
+        gx[e] = acc;
+    }
+}
+
 static inline int grid_for(long long work_items, int per_block) {
     long long blocks = (work_items + per_block - 1) / per_block;
     const long long cap = static_cast<long long>(kNumSMs) * 16;  // multiple of the SM count; grid-stride beyond
@@ -1186,6 +1257,23 @@ int gifb200_cond_down(float* x, float* y, int B, int H, int W, int C, int s, int
         const long long total = static_cast<long long>(B) * H * W * C;
         cond_down_adj_kernel<<<grid_for(total, 256), 256, 0, st>>>(x, y, B, H, W, C, s);
         GIFB200_LAUNCH_CHECK("cond_down_adj_kernel");
+    }
+    return GIFB200_OK;
+}
+
+int gifb200_cond_up(float* x, float* y, int B, int H, int W, int C, int s, int adjoint, gifb200_stream_t stream) {
+    GIFB200_REQUIRE(B >= 0 && H > 0 && W > 0 && C > 0, GIFB200_E_SHAPE, "cond_up: bad shape");
+    GIFB200_REQUIRE(s >= 2 && (s & (s - 1)) == 0, GIFB200_E_SHAPE, "cond_up: s must be a power of two >= 2");
+    if (B == 0) return GIFB200_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!adjoint) {
+        const long long total = static_cast<long long>(B) * H * s * W * s * C;
+        cond_up_kernel<<<grid_for(total, 256), 256, 0, st>>>(x, y, B, H, W, C, s);
+        GIFB200_LAUNCH_CHECK("cond_up_kernel");
+    } else {
+        const long long total = static_cast<long long>(B) * H * W * C;
+        cond_up_adj_kernel<<<grid_for(total, 256), 256, 0, st>>>(x, y, B, H, W, C, s);
+        GIFB200_LAUNCH_CHECK("cond_up_adj_kernel");
     }
     return GIFB200_OK;
 }

@@ -76,8 +76,7 @@ def _synth_from_w(g, w, cond, step):
     """Runs the synthesis network of a StyledGenerator from a given w (B,512) with the condition pyramid."""
     from . import ops
     c = ops.to_nhwc(cond)
-    full = c.shape[1]
-    noise = [ops.to_nchw_view(ops.cond_down(c, full // (4 * 2 ** i))) for i in range(step + 1)]
+    noise = [ops.to_nchw_view(ops.cond_resize(c, 4 * 2 ** i)) for i in range(step + 1)]
     return g.generator([w], None, noise, step, 1)[0]
 
 

@@ -168,16 +168,11 @@ class StyledGenerator(nn.Module):
         if noise is None:
             noise = [torch.zeros(batch, 3, 4 * 2 ** i, 4 * 2 ** i, device=input[0].device) for i in range(step + 1)]
         if self.rendered_flame_ascondition or self.normal_maps_as_cond:
-            # condition pyramid (gen.py:309-314): bilinear, align_corners=False, power-of-two reductions
+            # condition pyramid (gen.py:309-314): bilinear, align_corners=False, power-of-two reductions and enlargements
             cond = ops.to_nhwc(input[0])
-            full = cond.shape[1]
             noise = list(noise)
             for i in range(step + 1):
-                size = 4 * 2 ** i
-                if full % size != 0 or (full // size) & (full // size - 1):
-                    raise NotImplementedError("gif_b200 condition pyramid: the condition resolution must be a "
-                                              f"power-of-two multiple of every level (got {full} -> {size})")
-                noise[i] = ops.to_nchw_view(ops.cond_down(cond, full // size))
+                noise[i] = ops.to_nchw_view(ops.cond_resize(cond, 4 * 2 ** i))
         if mean_style is not None:
             styles = [mean_style + style_weight * (style - mean_style) for style in styles]
         return self.generator(styles, pose, noise, step, alpha, input_indices=input_indices, mixing_range=mixing_range)

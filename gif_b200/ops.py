@@ -994,6 +994,46 @@ def cond_down(x, s):
     return _CondDown.apply(x, s, False, tuple(x.shape[1:3]))
 
 
+class _CondUp(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, s, adjoint, small_hw):
+        x = _c(x)
+        require_cuda(x)
+        B, _, _, C = x.shape
+        H, W = small_hw
+        if not adjoint:
+            y = torch.empty((B, H * s, W * s, C), dtype=torch.float32, device=x.device)
+            check(lib.gifb200_cond_up(ptr(x), ptr(y), B, H, W, C, s, 0, stream()), "gifb200_cond_up")
+        else:
+            y = torch.empty((B, H, W, C), dtype=torch.float32, device=x.device)
+            check(lib.gifb200_cond_up(ptr(y), ptr(x), B, H, W, C, s, 1, stream()), "gifb200_cond_up(adj)")
+        ctx.cfg = (s, adjoint, small_hw)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        s, adjoint, small_hw = ctx.cfg
+        return _CondUp.apply(g, s, not adjoint, small_hw), None, None, None
+
+
+def cond_up(x, s):
+    """(B,H,W,C) -> (B,sH,sW,C): bilinear (align_corners=False) upsampling by a power of two, edges clamped as torch does."""
+    if s == 1:
+        return x
+    return _CondUp.apply(x, s, False, tuple(x.shape[1:3]))
+
+
+def cond_resize(x, size):
+    """(B,H,W,C) -> (B,size,size,C) for a square power-of-two ratio: F.interpolate(x, (size, size), 'bilinear',
+    align_corners=False) (gen.py:309-314).  Other ratios raise NotImplementedError."""
+    full = x.shape[1]
+    big, small = max(full, size), min(full, size)
+    if x.shape[2] != full or big % small != 0 or (big // small) & (big // small - 1):
+        raise NotImplementedError("gif_b200 condition pyramid: the condition and every level must differ by a power-of-two "
+                                  f"factor (got {tuple(x.shape[1:3])} -> {size})")
+    return cond_down(x, full // size) if full >= size else cond_up(x, size // full)
+
+
 # --------------------------------------------------------------------------------------------- layout helpers
 class _BoundaryIn(torch.autograd.Function):
     """NCHW tensor coming from reference-side code -> contiguous channels-last (B,H,W,C).  Same values as ``to_nhwc``; the

@@ -200,6 +200,11 @@ int gifb200_sgemm(int transA, int transB, int M, int N, int K, float alpha, cons
  * adjoint != 0 computes the transpose map (y given, x produced, zeros elsewhere). */
 int gifb200_cond_down(float* x, float* y, int B, int H, int W, int C, int s, int adjoint,
                       gifb200_stream_t stream);
+/* Upsampling counterpart (a 256^2 condition feeding the 512^2 / 1024^2 levels): F.interpolate(bilinear,
+ * align_corners=False) by a power of two s >= 2, edges clamped as torch does.  x (B,H,W,C) -> y (B,sH,sW,C); adjoint != 0
+ * computes the transpose map (y given, x produced). */
+int gifb200_cond_up(float* x, float* y, int B, int H, int W, int C, int s, int adjoint,
+                    gifb200_stream_t stream);
 
 /* ---- rasteriser ---------------------------------------------------------------------------------------
  * Replaces standard_rasterize / standard_rasterize_colors
