@@ -10,10 +10,12 @@ same class / method names and return values, with the statistics kept ON THE DEV
     (fid_score.py:176): same value for positive semi-definite covariances, no complex round trip.
 
 The feature extractor is the FID Inception network of pytorch_fid (torchvision's InceptionV3 with the FID weights,
-pt_inception-2015-12-05): weights are not in this image, so the model is INJECTED (any module mapping (B,3,H,W) in [0,1] to
-a list whose first element is (B,C,h,w) features, which is the interface of pytorch_fid.InceptionV3); its convolutions are
-library code (cuDNN through torch) -- this row is "next" scope, the generator side of the loop is
-gif_b200/inference.py."""
+pt_inception-2015-12-05).  ``FidComputer(inception_weights=...)`` builds ``gif_b200.inception.InceptionV3`` -- the network on
+this library's own kernels (general-geometry convolution, pooling, bilinear resize), forward only, in the precision of
+``ops.set_precision`` -- from a weights path or state dict (``inception_weights=True``: the standard file under
+$TORCH_HOME; it is never downloaded).  A model can still be INJECTED instead (any module mapping (B,3,H,W) in [0,1] to a list
+whose first element is (B,C,h,w) features, which is the interface of pytorch_fid.InceptionV3).  The generator side of the
+loop is gif_b200/inference.py."""
 import os
 
 import numpy as np
@@ -75,12 +77,19 @@ def compute_activation_batch(model, batch):
 
 
 class FidComputer:
-    """compute_fid.py:10-87.  ``model``: the FID Inception network (see the module docstring); ``true_img_stats_dir`` holds the
-    reference's ``ffhq_{R}X{R}_fid_stats.npz`` files (mu, sigma)."""
+    """compute_fid.py:10-87.  ``model``: the FID Inception network, or None with ``inception_weights`` to build the native one
+    for ``dims`` (see the module docstring); ``true_img_stats_dir`` holds the reference's ``ffhq_{R}X{R}_fid_stats.npz`` files
+    (mu, sigma)."""
 
-    def __init__(self, database_root_dir=None, true_img_stats_dir=None, model=None, dims=2048, device=None):
+    def __init__(self, database_root_dir=None, true_img_stats_dir=None, model=None, dims=2048, device=None,
+                 inception_weights=None):
         if model is None:
-            raise ValueError("FidComputer needs the FID Inception network (pytorch_fid.InceptionV3 with its weights): pass model=...")
+            if inception_weights is None:
+                raise ValueError("FidComputer needs the FID Inception network: pass model=... (e.g. pytorch_fid.InceptionV3) "
+                                 "or inception_weights=<path or state dict> (True: search $TORCH_HOME)")
+            from .inception import InceptionV3
+            model = InceptionV3([InceptionV3.BLOCK_INDEX_BY_DIM[dims]],
+                                weights=None if inception_weights is True else inception_weights)
         self.dims = dims
         self.true_data_loc = database_root_dir
         self.true_img_stats_dir = true_img_stats_dir

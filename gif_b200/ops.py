@@ -1034,6 +1034,105 @@ def cond_resize(x, size):
     return cond_down(x, full // size) if full >= size else cond_up(x, size // full)
 
 
+# --------------------------------------------------------------------------------------------- forward-only feature network ops
+# The FID Inception network never needs gradients: these wrappers take no part in autograd and refuse inputs that require
+# grad (under grad mode) instead of silently returning a result without a graph.
+def _forward_only(what, *tensors):
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
+        raise RuntimeError(f"gif_b200.ops.{what} is forward-only: its inputs must not require grad")
+
+
+def conv_ex_out_size(h, k, stride, pad):
+    return (h + 2 * pad - k) // stride + 1
+
+
+def conv2d_ex_impl(x_shape, co, kh, kw, stride, pad):
+    """The gifb200_conv2d_ex impl the current precision mode runs for this shape: 1 (exact fp32), 2 (tf32) or 3 (bf16x3)."""
+    if CONV_IMPL == 1:
+        return 1
+    B, Hi, Wi, Ci = x_shape
+    Ho, Wo = conv_ex_out_size(Hi, kh, stride, pad[0]), conv_ex_out_size(Wi, kw, stride, pad[1])
+    if lib.gifb200_conv2d_ex_workspace_bytes(B, Hi, Wi, Ci, Ho, Wo, co, kh, kw, stride, pad[0], pad[1], 2) == 0:
+        return 1
+    return 3 if CONV_IMPL == 3 else 2
+
+
+def conv2d_ex(x, w, kh, kw, stride=1, pad=(0, 0), bias=None, relu=False, out=None, c0=0, round_tf32=False, workspace=None):
+    """Forward-only general convolution (gifb200_conv2d_ex): x (B,H,W,Ci) channels-last, w (kh*kw, Co, Ci) tap-major,
+    y = relu?(conv(x, w) + bias).  ``out`` (B,Ho,Wo,Cy): write channels [c0, c0+Co) of it instead of a new tensor.
+    The precision mode (``set_precision``) picks the kernel; tensor-core inputs are rounded to tf32 or split into bf16
+    planes (cached per tensor) here.  ``workspace``: a caller-kept ``[tensor or None, staged impl]`` list holding the staged
+    weights of ``w`` between calls (GIFB200_CONV_PRESTAGED); None stages ``w`` on every call."""
+    _forward_only("conv2d_ex", x, w, bias)
+    require_cuda(x, w, bias)
+    x = _c(x)
+    B, Hi, Wi, Ci = x.shape
+    T, Co, Ci_w = w.shape
+    if T != kh * kw or Ci_w != Ci:
+        raise ValueError(f"conv2d_ex: weight {tuple(w.shape)} vs kernel {kh}x{kw} and input channels {Ci}")
+    if bias is not None and not relu:
+        raise ValueError("conv2d_ex: the fused epilogue is bias + ReLU; a bias needs relu=True")
+    Ho, Wo = conv_ex_out_size(Hi, kh, stride, pad[0]), conv_ex_out_size(Wi, kw, stride, pad[1])
+    if out is None:
+        out = torch.empty((B, Ho, Wo, Co), dtype=torch.float32, device=x.device)
+    elif out.shape[:3] != (B, Ho, Wo) or not out.is_contiguous() or out.dtype != torch.float32:
+        raise ValueError(f"conv2d_ex: out {tuple(out.shape)} is not a contiguous (B, {Ho}, {Wo}, Cy) float32 tensor")
+    impl = conv2d_ex_impl(x.shape, Co, kh, kw, stride, pad)
+    xin = x
+    if impl == 3:
+        xin = _planes(x)
+    elif impl == 2 and not _is_tf32(x):
+        xin = _tag(_round_tf32_raw(x), True)
+    nws = lib.gifb200_conv2d_ex_workspace_bytes(B, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad[0], pad[1], impl)
+    flag = 0
+    if nws == 0:
+        ws = None
+    elif workspace is None:
+        ws = _workspace(nws, x.device)
+    else:
+        if workspace[0] is None or workspace[0].numel() < nws or workspace[1] != impl:
+            workspace[0], workspace[1] = torch.empty(nws, dtype=torch.uint8, device=x.device), impl
+        else:
+            flag = 0x10                                      # GIFB200_CONV_PRESTAGED: the staged weights are current
+        ws = workspace[0]
+    check(lib.gifb200_conv2d_ex(ptr(xin), ptr(_c(w)), ptr(out), B, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad[0], pad[1],
+                                out.shape[3], c0, impl | flag, int(relu), ptr(bias), int(round_tf32),
+                                ptr(ws), nws, stream()), "gifb200_conv2d_ex")
+    return out
+
+
+def pool2d(x, op, stride, pad, out=None, c0=0, round_tf32=False):
+    """Forward-only 3x3 pooling (gifb200_pool2d) of x (B,H,W,C): op "max" (padded cells -inf) or "avg"
+    (count_include_pad=False); ``out``/``c0`` as in conv2d_ex."""
+    _forward_only("pool2d", x)
+    require_cuda(x)
+    x = _c(x)
+    B, Hi, Wi, C = x.shape
+    Ho, Wo = conv_ex_out_size(Hi, 3, stride, pad), conv_ex_out_size(Wi, 3, stride, pad)
+    if out is None:
+        out = torch.empty((B, Ho, Wo, C), dtype=torch.float32, device=x.device)
+    elif out.shape[:3] != (B, Ho, Wo) or not out.is_contiguous():
+        raise ValueError(f"pool2d: out {tuple(out.shape)} is not a contiguous (B, {Ho}, {Wo}, Cy) tensor")
+    check(lib.gifb200_pool2d(ptr(x), ptr(out), B, Hi, Wi, C, Ho, Wo, stride, pad, {"max": 0, "avg": 1}[op], out.shape[3], c0,
+                             int(round_tf32), stream()), "gifb200_pool2d")
+    return out
+
+
+def resize_bilinear(x, size, channels=32, scale=1.0, shift=0.0, round_tf32=False):
+    """Forward-only F.interpolate(x, size, 'bilinear', align_corners=False) then scale*v + shift (gifb200_resize_bilinear):
+    x (B,3,H,W) fp32 with any strides -> channels-last (B,size[0],size[1],channels), channels 3.. zero."""
+    _forward_only("resize_bilinear", x)
+    require_cuda(x)
+    B, C, H, W = x.shape
+    if C != 3:
+        raise ValueError(f"resize_bilinear takes (B,3,H,W) images, got {tuple(x.shape)}")
+    y = torch.empty((B, size[0], size[1], channels), dtype=torch.float32, device=x.device)
+    sb, sc, sh, sw = x.stride()
+    check(lib.gifb200_resize_bilinear(ptr(x), ptr(y), B, H, W, sb, sc, sh, sw, size[0], size[1], channels, float(scale),
+                                      float(shift), int(round_tf32), stream()), "gifb200_resize_bilinear")
+    return y
+
+
 # --------------------------------------------------------------------------------------------- layout helpers
 class _BoundaryIn(torch.autograd.Function):
     """NCHW tensor coming from reference-side code -> contiguous channels-last (B,H,W,C).  Same values as ``to_nhwc``; the

@@ -98,6 +98,39 @@ int gifb200_conv2d_wgrad(const float* x, const float* gy, float* gw, int B, int 
                          int Co, int k, int mode, int flip, int transposed, int impl, void* workspace,
                          size_t workspace_bytes, gifb200_stream_t stream);
 
+/* ---- general-geometry forward convolution (FID InceptionV3) ---------------------------------------------
+ * Replaces the nn.Conv2d (bias-free) + BatchNorm2d (folded into w and bias by the caller) + ReLU of torchvision's BasicConv2d
+ * as my_utils/pytorch_fid/inception.py uses it (FID feature network, my_utils/compute_fid.py):
+ *     y[b,yo,xo,c0+o] = act(sum_{kh',kw',i} x[b, yo*stride - pad_h + kh', xo*stride - pad_w + kw', i] * w[kh'*kw + kw'][o][i]
+ *                           + bias[o])
+ * with zero padding; act == 1: ReLU (bias may be NULL), act == 0: the plain sum.  round_tf32 != 0 rounds y to tf32.
+ * x (B,Hi,Wi,Ci) dense channels-last; w tap-major [kh*kw][Co][Ci]; y has Cy channels per pixel and only channels
+ * [c0, c0+Co) are written (the branches of an Inception block write their slices of the concatenation).
+ * Geometry: 1 <= kh, kw <= 7, stride 1 or 2, pad_h, pad_w >= 0, any sizes with (Ho-1)*stride + kh <= Hi + 2*pad_h (same in x).
+ * impl as gifb200_conv2d: 1 exact fp32 SIMT, 2 wgmma tf32 (x must be tf32-representable), 3 wgmma bf16x3 (x is the planes
+ * buffer of gifb200_split_bf16), 0 auto (2 when the shape qualifies, else 1).  The tensor-core paths need Ci % 32 == 0,
+ * Co % 32 == 0, even Cy and c0, x 16-byte and y 8-byte aligned (callers pad channels with zero weights and zero bias: the
+ * padded outputs are exactly 0).  GIFB200_CONV_PRESTAGED may be OR-ed into impl as for gifb200_conv2d.
+ * workspace: gifb200_conv2d_ex_workspace_bytes(...) (0 for the SIMT path): the staged weights, then -- when the output
+ * tiles cannot fill the machine -- split-K partial sums, added in a fixed order (deterministic). */
+size_t gifb200_conv2d_ex_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, int Wo, int Co, int kh, int kw, int stride,
+                                         int pad_h, int pad_w, int impl);
+int gifb200_conv2d_ex(const void* x, const float* w, float* y, int B, int Hi, int Wi, int Ci, int Ho, int Wo, int Co, int kh,
+                      int kw, int stride, int pad_h, int pad_w, int Cy, int c0, int impl, int act, const float* bias,
+                      int round_tf32, void* workspace, size_t workspace_bytes, gifb200_stream_t stream);
+/* 3x3 pooling of x (B,Hi,Wi,C) into channels [c0, c0+C) of y (B,Ho,Wo,Cy): op 0 = max (padded cells are -inf, as
+ * F.max_pool2d), op 1 = average with count_include_pad=False (FIDInceptionA/C/E_1's F.avg_pool2d); stride 1 or 2,
+ * pad 0 or 1.  Replaces nn.MaxPool2d(3, 2) / F.max_pool2d / F.avg_pool2d of my_utils/pytorch_fid/inception.py. */
+int gifb200_pool2d(const float* x, float* y, int B, int Hi, int Wi, int C, int Ho, int Wo, int stride, int pad, int op, int Cy,
+                   int c0, int round_tf32, gifb200_stream_t stream);
+/* F.interpolate(x, size=(Ho,Wo), mode='bilinear', align_corners=False) followed by v -> scale*v + shift
+ * (InceptionV3.forward's resize and normalize_input, my_utils/pytorch_fid/inception.py:147-154).  x (B,3,H,W) is read through
+ * its element strides (NCHW-contiguous or the NCHW view of channels-last storage); y (B,Ho,Wo,Cy) channels-last with
+ * channels 3..Cy-1 set to 0. */
+int gifb200_resize_bilinear(const float* x, float* y, int B, int H, int W, long long stride_b, long long stride_c,
+                            long long stride_h, long long stride_w, int Ho, int Wo, int Cy, float scale, float shift,
+                            int round_tf32, gifb200_stream_t stream);
+
 /* Two-term bf16 expansion of an fp32 tensor (B, P pixels, C channels, channels-last), optionally fused with the style
  * modulation of ModulatedConv2d (cl.py:311-313 in the modulate-input form): v = x[b,p,c] * (s ? s[b,c] : 1);
  *     planes[0][b,p,c] = bf16_rn(v);   planes[1][b,p,c] = bf16_rn(v - planes[0][b,p,c])
