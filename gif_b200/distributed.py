@@ -190,5 +190,9 @@ def broadcast_module(module, src=0):
     """Make all replicas start from rank `src`'s parameters and buffers."""
     if not dist.is_initialized() or dist.get_world_size() == 1:
         return
-    for t in list(module.parameters()) + list(module.buffers()):
-        dist.broadcast(t.data, src)
+    ts = list(module.parameters()) + list(module.buffers())
+    with torch.no_grad():
+        for t in ts:
+            dist.broadcast(t, src)
+    # the collective writes in place without bumping the version counters (which the prepared-weight cache keys on)
+    torch.autograd.graph.increment_version(ts)

@@ -134,7 +134,7 @@ class EqualConv2d(nn.Module):
 
     def forward_nhwc(self, x):
         mode = _conv_mode(self.kernel_size, self.stride, self.padding)
-        wt = ops.prep_weight(self.weight, self.scale)
+        wt = ops.prep_weight(self.weight, self.scale, cache=self.training)
         x, wt = _pad_channels_for_tc(x, wt)
         if self.bias is not None:
             return ops.conv2d_bias_act(x, wt, self.bias, self.kernel_size, mode, slope=1.0, gain=1.0)
@@ -223,7 +223,7 @@ class ModulatedConv2d(nn.Module):
         """NHWC x -> (acc, d): the un-demodulated shared-weight convolution of the modulated input (after the blur
         of the upsample branch) and the demodulation coefficients d[b,o] (None if demodulate=False)."""
         s = self.modulation(style)                                        # (B,Ci)  cl.py:311
-        wt = ops.prep_weight(self.weight[0], self.scale)                  # (T,Co,Ci) = W~ tap-major
+        wt = ops.prep_weight(self.weight[0], self.scale, cache=self.training)   # (T,Co,Ci) = W~ tap-major
         k = self.kernel_size
         if k == 1 and self.out_channel == 3 and not (self.upsample or self.downsample):
             # ToRGB: per-sample 1x1 weights ws[b,c,i] = W~[c,i] s[b,i] (3*Ci numbers per sample), no modulated copy of x
@@ -282,7 +282,7 @@ class NoiseInjection(nn.Module):
         the values are unchanged) which makes all three convolutions eligible for the tensor-core kernel: 5x more nominal
         FLOPs on the first one, but on a pipe that is ~50x faster than the fp32 SIMT path."""
         c0, c2, c4 = self.noise_conv[0], self.noise_conv[2], self.noise_conv[4]
-        w0, w2, w4 = ops.prep_weight(c0.weight), ops.prep_weight(c2.weight), ops.prep_weight(c4.weight)
+        w0, w2, w4 = (ops.prep_weight(c.weight, cache=self.training) for c in (c0, c2, c4))
         b0, b2 = c0.bias, c2.bias
         if ops.tc_enabled() and noise.shape[1] >= 4 and (noise.shape[1] & (noise.shape[1] - 1)) == 0:
             def up32(n):
@@ -507,7 +507,7 @@ class ConvLayer(nn.Sequential):
         act = layers[i + 1] if i + 1 < len(layers) else None
         k = conv.kernel_size
         mode = ops.S1 if (k == 1 and conv.stride == 2) else _conv_mode(k, conv.stride, conv.padding)
-        xp, wt = _pad_channels_for_tc(x, ops.prep_weight(conv.weight, conv.scale))
+        xp, wt = _pad_channels_for_tc(x, ops.prep_weight(conv.weight, conv.scale, cache=self.training))
         if isinstance(act, FusedLeakyReLU):
             return ops.conv2d_bias_act(xp, wt, act.bias, k, mode, act.negative_slope, act.scale, rt=rt_out and tf32)
         if isinstance(act, ScaledLeakyReLU):

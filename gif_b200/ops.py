@@ -368,7 +368,8 @@ def conv2d(x, w, k, mode=S1, flip=False, transposed=False):
 
 
 _NO_WEIGHT_CACHE = bool(os.environ.get("GIFB200_NO_WEIGHT_CACHE"))    # A/B switch: recompute the tap-major weights on every call
-_prep_cache = {}     # (id of the parameter, view offset, shape, scale) -> (weakref to the parameter, its version, buffer, serial)
+_prep_cache = {}     # (id of the parameter, view offset, shape, scale) -> (weakref to the parameter, its version, buffer, serial,
+                     #                                                  address of the weight)
 _stage_cache = {}    # (prep key, flip, transposed, impl, conv shape) -> [prep serial it was staged from, persistent workspace]
 _prep_serial = [0]   # bumped on every recomputation: what the staged-operand cache compares (immune to address / id reuse)
 
@@ -390,13 +391,14 @@ class _PrepWeight(torch.autograd.Function):
         key = (id(base), weight.storage_offset(), (co, ci, kh, kw), float(scale))
         hit = _prep_cache.get(key)
         # identity is checked through a weak reference: ids and addresses are reused once a network is freed, and a new
-        # parameter that lands on an old one's id with an equal version counter must not see its prepared weights
-        if hit is None or hit[0]() is not base or hit[1] != weight._version:
+        # parameter that lands on an old one's id with an equal version counter must not see its prepared weights.
+        # ``p.data = t`` rebinds the parameter to other storage without bumping its version: the address tells.
+        if hit is None or hit[0]() is not base or hit[1] != weight._version or hit[4] != weight.data_ptr():
             same = hit is not None and hit[0]() is base
             buf = hit[2] if same else torch.empty((kh * kw, co, ci), dtype=torch.float32, device=weight.device)
             torch.mul(weight.detach().permute(2, 3, 0, 1), scale, out=buf.view(kh, kw, co, ci))    # one kernel, in place
             _prep_serial[0] += 1
-            hit = (weakref.ref(base), weight._version, buf, _prep_serial[0])
+            hit = (weakref.ref(base), weight._version, buf, _prep_serial[0], weight.data_ptr())
             _prep_cache[key] = hit
             if len(_prep_cache) > 4096:                                        # entries of freed networks
                 for k_ in [k_ for k_, v_ in _prep_cache.items() if v_[0]() is None]:
@@ -413,9 +415,12 @@ class _PrepWeight(torch.autograd.Function):
         return (g.reshape(kh, kw, co, ci) * scale).permute(2, 3, 0, 1), None
 
 
-def prep_weight(weight, scale=1.0):
-    """(Co,Ci,k,k) parameter -> tap-major (k*k, Co, Ci) * scale (differentiable; cached per parameter version)."""
-    if weight.is_cuda and weight.dtype == torch.float32 and not _NO_WEIGHT_CACHE:
+def prep_weight(weight, scale=1.0, cache=True):
+    """(Co,Ci,k,k) parameter -> tap-major (k*k, Co, Ci) * scale (differentiable; cached per parameter version).
+    cache=False (the layers pass ``self.training``): prepare and stage on every call.  An eval-mode copy such as the EMA
+    generator is updated by code that writes through ``.data`` (the reference's ``accumulate``), which no version counter
+    sees."""
+    if cache and weight.is_cuda and weight.dtype == torch.float32 and not _NO_WEIGHT_CACHE:
         return _PrepWeight.apply(weight, float(scale))
     co, ci, kh, kw = weight.shape
     return (weight * scale).permute(2, 3, 0, 1).reshape(kh * kw, co, ci).contiguous()
@@ -431,6 +436,8 @@ def _staged_workspace(w, nws, flip, transposed, impl, shape_key, device):
     key = (pkey, bool(flip), bool(transposed), impl, shape_key)
     ent = _stage_cache.get(key)
     if ent is None or ent[1].numel() < nws:
+        if ent is not None:
+            _ws_retired.append(ent[1])           # retired, never freed: a captured CUDA graph may hold its address
         ent = [None, torch.empty(nws, dtype=torch.uint8, device=device)]
         _stage_cache[key] = ent
     fresh = ent[0] == serial

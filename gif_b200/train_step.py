@@ -34,11 +34,12 @@ def requires_grad(model, flag=True):
 
 
 def accumulate(model1, model2, decay=0.999):
-    """my_utils/generic_utils.py:63-76 (EMA), as one fused foreach update."""
-    p1 = [p.data for p in model1.parameters()]
-    p2 = [p.data for p in model2.parameters()]
-    torch._foreach_mul_(p1, decay)
-    torch._foreach_add_(p1, p2, alpha=1 - decay)
+    """my_utils/generic_utils.py:63-76 (EMA), as one fused foreach update.  Written under no_grad rather than through
+    ``.data``, so that the parameters' version counters (which the prepared-weight cache keys on) see the write."""
+    with torch.no_grad():
+        p1, p2 = list(model1.parameters()), list(model2.parameters())
+        torch._foreach_mul_(p1, decay)
+        torch._foreach_add_(p1, p2, alpha=1 - decay)
 
 
 class GifTrainer:
@@ -129,6 +130,8 @@ class GifTrainer:
             self.graph_launches[with_r1] = _lib.launch_count() - n0      # gif_b200 kernel nodes per replayed iteration
             graphs[with_r1] = (segs, (state["d_loss"], state["g_loss"]))
         self._graphs = graphs
+        # a replay writes the parameters without running Python, so their version counters do not move: bumped by hand
+        self._replay_written = [p for m in (self.generator, self.discriminator, self.g_running) for p in m.parameters()]
 
     def train_iteration(self, real_image, flm_rndr, input_indices, flm_lbls=None):
         """real_image (B,3,R,R) in [-1,1], flm_rndr (B,6,R,R) in [-1,1], input_indices (B,) int64 -- device tensors (or
@@ -147,6 +150,7 @@ class GifTrainer:
             g2.replay()
             self.g_reducer.reduce()
             g3.replay()
+            torch.autograd.graph.increment_version(self._replay_written)
             return out
         state = {}
         self._seg1(state, real_image, flm_rndr, input_indices, with_r1)
