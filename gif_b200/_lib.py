@@ -64,6 +64,11 @@ SIGNATURES = {
     "gifb200_flame_lbs": (_i, [_p] * 11 + [_i] * 4 + [_p, _sz, _p]),
     "gifb200_texture_steal_fwd": (_i, [_p] * 9 + [_i] * 6 + [_p]),
     "gifb200_texture_steal_bwd": (_i, [_p] * 7 + [_i] * 6 + [_p]),
+    "gifb200_jpeg_workspace_bytes": (_sz, [_i, _i, _ll]),
+    "gifb200_jpeg_decode": (_i, [_p] * 6 + [_i, _i, _i, _ll, _i, _i, _p, _p, _p, _sz, _p]),
+    "gifb200_png_unfilter": (_i, [_p, _p, _i, _i, _p, _p, _p]),
+    "gifb200_resize_bicubic_u8": (_i, [_p] * 5 + [_i] * 7 + [_p]),
+    "gifb200_u8_to_unit": (_i, [_p, _p, _i, _i, _i, _ll, _p]),
 }
 
 

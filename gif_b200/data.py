@@ -358,3 +358,151 @@ class PinnedBatchLoader:
                 return
             yield buf
             free.put(buf)       # the consumer is done with the previous batch once it asks for the next one
+
+
+class DeviceBatchLoader:
+    """Batches of a GifLmdbDataset decoded on the device (gif_b200.image_decode), bitwise equal to ``PinnedBatchLoader``'s
+    with the same order, seed handling and drop_last.  Real images must be baseline JPEG and renders 8-bit PNG, as the
+    reference's LMDB writers store them; anything else raises ``UnsupportedImage`` naming the key.
+
+    A background thread reads the raw LMDB values, parses them, inflates the PNGs on a small thread pool and fills a pinned
+    byte arena.  The consuming thread enqueues one non-blocking copy of the arena plus the decode kernels on a side stream,
+    one batch ahead, so batch k+1 decodes while the caller trains on batch k.  It yields device tensors (real (B,3,R,R),
+    cond (B,6,R,R), labels (B,P), indices (B,) int64) -- the arguments of ``GifTrainer.train_iteration`` -- after making the
+    current stream wait for their decode.  Each batch stays valid until the next one is requested.  Before yielding a batch
+    it waits for that batch's decode (queued a step earlier on the side stream, never behind training work) and reads its
+    per-image status words, so a corrupt image raises before its batch is used."""
+
+    def __init__(self, dataset, batch_size, shuffle=True, seed=0, depth=3, device=None, threads=4):
+        self.ds, self.bs, self.shuffle, self.seed, self.depth = dataset, batch_size, shuffle, seed, depth
+        self.device = torch.device(device or "cuda")
+        self.threads = threads
+        self.pin = torch.cuda.is_available()
+        self._stream = None
+
+    def _host_batch(self, ids, pool):
+        from . import image_decode as I
+        ds, R, rr = self.ds, self.ds.resolution, self.ds.rend_flm_res
+        keys = [image_key(R, i) for i in ids]
+        rkeys = [image_key(rr, i) for i in ids] + [normal_map_key(rr, i) for i in ids]
+
+        def png(k):
+            try:
+                h = I.parse_png(ds.rend.get(k))
+                if (h[0], h[1]) != (rr, rr):
+                    raise I.UnsupportedImage(f"{h[0]}x{h[1]} render, rend_flm_res is {rr}")
+                return h, I.inflate_png(h)
+            except I.UnsupportedImage as e:
+                raise I.UnsupportedImage(f"{k.decode()}: {e}") from None
+        pngs = pool.map(png, rkeys)                 # inflates on the pool while this thread parses the JPEGs
+        parsed = []
+        for k in keys:
+            try:
+                p = I.parse_jpeg(ds.real.get(k))
+            except I.UnsupportedImage as e:
+                raise I.UnsupportedImage(f"{k.decode()}: {e}") from None
+            if (p["w"], p["h"]) != (R, R):
+                raise I.UnsupportedImage(f"{k.decode()}: {p['w']}x{p['h']} real image, the dataset's resolution is {R}")
+            parsed.append(p)
+        pngs = list(pngs)
+        jb = I.JpegBatch(parsed)
+        pb = I.PngBatch([h for h, _ in pngs], [r for _, r in pngs])
+        sizes = [len(jb.data), pb.data_bytes, 4 * jb.ints.size, 4 * pb.desc.size]
+        offs = np.concatenate([[0], np.cumsum([(s + 255) // 256 * 256 for s in sizes])])
+        arena = torch.empty(int(offs[-1]), dtype=torch.uint8, pin_memory=self.pin)
+        a = arena.numpy()
+        a[:sizes[0]] = np.frombuffer(jb.data, np.uint8)
+        o = offs[1]
+        for _, r in pngs:
+            a[o:o + len(r)] = np.frombuffer(r, np.uint8)
+            o += len(r)
+        a[offs[2]:offs[2] + sizes[2]] = jb.ints.view(np.uint8)
+        a[offs[3]:offs[3] + sizes[3]] = pb.desc.ravel().view(np.uint8)
+        lbl = np.stack([(ds.flame_params[i] - ds.flame_mean) / ds.flame_std for i in ids]).astype(np.float32)
+        pin = (lambda t: t.pin_memory()) if self.pin else (lambda t: t)
+        return arena, offs, jb, pb, pin(torch.from_numpy(lbl)), pin(torch.tensor(ids, dtype=torch.int64)), keys, rkeys
+
+    def _launch(self, hb):
+        """Enqueue the copy and the decode of one host batch on the side stream."""
+        from . import image_decode as I
+        arena, offs, jb, pb, lbl, idx, keys, rkeys = hb
+        dev, B, R, rr = self.device, self.bs, self.ds.resolution, self.ds.rend_flm_res
+        with torch.cuda.stream(self._stream):
+            d = arena.to(dev, non_blocking=True)
+            seg = lambda i: d[int(offs[i]):int(offs[i + 1])]
+            status = torch.zeros(3 * B, dtype=torch.int32, device=dev)
+            real_u8 = torch.empty(B, R, R, 3, dtype=torch.uint8, device=dev)
+            rend_u8 = torch.empty(2 * B, rr, rr, 3, dtype=torch.uint8, device=dev)
+            ws = torch.empty(jb.workspace_bytes, dtype=torch.uint8, device=dev)
+            jb.launch(seg(0), seg(2), real_u8, status[:B], ws)
+            pb.launch(seg(1), seg(3), rend_u8, status[B:])
+            if rr != R:
+                rend_u8 = I.resize_bicubic_u8(rend_u8, R)
+            real = torch.empty(B, 3, R, R, device=dev)
+            cond = torch.empty(B, 6, R, R, device=dev)
+            I.u8_to_unit(real_u8, real)
+            I.u8_to_unit(rend_u8[:B], cond[:, 0:3])
+            I.u8_to_unit(rend_u8[B:], cond[:, 3:6])
+            labels, indices = lbl.to(dev, non_blocking=True), idx.to(dev, non_blocking=True)
+            st = status.to("cpu", non_blocking=True) if self.pin else status.cpu()
+            done = torch.cuda.Event()
+            done.record()
+        return (real, cond, labels, indices), st, done, keys + rkeys
+
+    def _finish(self, launched):
+        from . import image_decode as I
+        out, st, done, keys = launched
+        done.synchronize()                          # the side stream only: this batch's copy and decode
+        bad = np.flatnonzero(st.numpy())
+        if bad.size:
+            raise I.UnsupportedImage(f"{keys[bad[0]].decode()}: corrupt or truncated image data "
+                                     f"(device status {int(st[bad[0]])})")
+        cur = torch.cuda.current_stream(self.device)
+        cur.wait_event(done)
+        for t in out:                               # allocated on the side stream, used on this one
+            t.record_stream(cur)
+        return out
+
+    def __iter__(self):
+        order = np.arange(len(self.ds))
+        if self.shuffle:
+            np.random.default_rng(self.seed).shuffle(order)
+            self.seed += 1
+        nb = len(order) // self.bs                                              # drop_last=True, dataset_loaders.py:395
+        if self._stream is None:
+            self._stream = torch.cuda.Stream(self.device)
+        ready = queue.Queue(maxsize=self.depth)
+        stop = threading.Event()
+
+        def work():
+            from concurrent.futures import ThreadPoolExecutor
+            with ThreadPoolExecutor(self.threads) as pool:
+                for b in range(nb):
+                    if stop.is_set():
+                        return
+                    ids = [int(self.ds.valid_ids[int(j)]) for j in order[b * self.bs:(b + 1) * self.bs]]
+                    try:
+                        item = self._host_batch(ids, pool)
+                    except Exception as e:          # handed to the consumer, which raises it
+                        item = e
+                    ready.put(item)
+                    if isinstance(item, Exception):
+                        return
+            ready.put(None)
+
+        def next_launched():
+            hb = ready.get()
+            if isinstance(hb, Exception):
+                raise hb
+            return None if hb is None else self._launch(hb)
+        threading.Thread(target=work, daemon=True).start()
+        try:
+            pending = next_launched()
+            while pending is not None:
+                ahead = next_launched()             # batch k+1 decodes on the side stream while batch k trains
+                yield self._finish(pending)
+                pending = ahead
+        finally:
+            stop.set()
+            while not ready.empty():
+                ready.get_nowait()

@@ -318,6 +318,45 @@ int gifb200_texture_steal_bwd(const float* g_tex, const float* verts, const floa
                               const int32_t* vid, const float* bary, float* g_src, int B, int H, int W, int C, int V, int T,
                               gifb200_stream_t stream);
 
+/* ---- image decoding (training inputs) -------------------------------------------------------------------
+ * Replaces: PIL's Image.open(...).convert("RGB") [+ .resize((R, R))] + ToTensor + Normalize in FFHQ.__getitem__
+ * (dataset_loaders.py:268-280, 128-137).  The host (gif_b200/image_decode.py) parses markers / chunks and packs
+ * int32 descriptors; every result is bit-exact with Pillow 12 (libjpeg-turbo defaults: islow IDCT, fancy upsampling).
+ *
+ * Baseline JPEG (SOF0/SOF1, 8-bit, Huffman, 1 or 3 components, luma 1x1/2x1/1x2/2x2 with 1x1 chroma, DRI).  data = the
+ * un-stuffed entropy-coded segments (one per restart interval); img_desc (n_img x GIFB200_JPEG_DESC_INTS), seg_desc
+ * (n_seg x GIFB200_JPEG_SEG_INTS), chunk_seg (n_chunk: the segment of each chunk_bytes piece of a segment),
+ * qtab (n_img x 3 x 64, natural order), htab (n_img x 4 x GIFB200_JPEG_HUFF_INTS).  Each chunk is entropy-decoded by its
+ * own thread, synchronised on (bit position, block in MCU, coefficient index).  out: uint8 RGB (H, W, 3) per image at
+ * its descriptor's offset.  status (n_img, zeroed by the caller): bit 0 an invalid Huffman code, bit 1 a segment whose
+ * blocks do not match its MCU count (truncated or corrupt data).  max_blocks = largest per-image block count. */
+#define GIFB200_JPEG_DESC_INTS 48
+#define GIFB200_JPEG_SEG_INTS 8
+#define GIFB200_JPEG_HUFF_INTS 804
+size_t gifb200_jpeg_workspace_bytes(int n_chunk, int n_seg, long long n_blocks);
+int gifb200_jpeg_decode(const uint8_t* data, const int32_t* img_desc, const int32_t* seg_desc, const int32_t* chunk_seg,
+                        const int32_t* qtab, const int32_t* htab, int n_img, int n_seg, int n_chunk, long long n_blocks,
+                        int max_blocks, int chunk_bytes, uint8_t* out, int32_t* status, void* ws, size_t ws_bytes,
+                        gifb200_stream_t stream);
+
+/* PNG scanline reconstruction (filters None/Sub/Up/Average/Paeth, bit depth 8, not interlaced).  data = the inflated IDAT
+ * stream of each image (filter byte + W*C bytes per row), reconstructed IN PLACE; desc (n_img x GIFB200_PNG_DESC_INTS):
+ * data offset, W, H, C (1 grey, 3 RGB, 4 RGBA), out offset.  out: uint8 RGB (H, W, 3), grey replicated, alpha dropped.
+ * status bit 2: a row with an unknown filter type.  max_pixels = largest W*H. */
+#define GIFB200_PNG_DESC_INTS 8
+int gifb200_png_unfilter(uint8_t* data, const int32_t* desc, int n_img, int max_pixels, uint8_t* out, int32_t* status,
+                         gifb200_stream_t stream);
+
+/* Pillow's Image.resize((Wo, Ho)) of uint8 RGB images (B, Hi, Wi, 3) -> (B, Ho, Wo, 3): horizontal pass into tmp
+ * (B, Hi, Wo, 3), then vertical.  coef_h (Wo x (ks_h + 2)) / coef_v (Ho x (ks_v + 2)) rows = [first tap, tap count,
+ * 22-bit fixed-point weights], computed by the host in float64 as Pillow's precompute_coeffs does. */
+int gifb200_resize_bicubic_u8(const uint8_t* x, uint8_t* tmp, uint8_t* y, const int32_t* coef_h, const int32_t* coef_v, int B,
+                              int Hi, int Wi, int Ho, int Wo, int ks_h, int ks_v, gifb200_stream_t stream);
+
+/* uint8 RGB (B, H, W, 3) -> y[b*y_batch_stride + c*H*W + p] = (v / 255 - 0.5) / 0.5 (float32, IEEE division): three
+ * channels of an NCHW batch, so a render and a normal map go straight into their slices of the condition tensor. */
+int gifb200_u8_to_unit(const uint8_t* x, float* y, int B, int H, int W, long long y_batch_stride, gifb200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

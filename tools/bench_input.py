@@ -1,0 +1,172 @@
+"""Input-pipeline measurement.
+
+1. Host CPU seconds per batch: ``GifLmdbDataset`` items (PIL decode, the work of PinnedBatchLoader's thread) and
+   DeviceBatchLoader's host side (LMDB read, parsing, PNG inflate on its pool).  ``time.process_time`` sums every thread
+   of the process; torch runs with one intra-op thread so that OpenMP workers spin-waiting inside the PIL path's small
+   float ops are not counted as decode work.
+2. Device decode time per batch (CUDA events), split into JPEG (for several entropy chunk sizes), PNG and resize, with
+   the bytes each pass reads.
+3. ``--trainer``: GifTrainer images/s at 256^2 batch 32 (bf16x3, CUDA graphs, no path-length term) fed by DeviceBatchLoader
+   against the same step fed from pinned host tensors, alternating, three runs of each.
+
+The synthetic LMDBs follow the reference's writers (JPEG q100 4:2:0 real images, PNG renders at 256^2).  Prints the card,
+its power limit and clocks read in the same run; writes JSON to --out."""
+import argparse
+import itertools
+import json
+import os
+import subprocess
+import sys
+import tempfile
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+
+
+def cpu_per_batch(fn, reps):
+    fn()
+    t0 = time.process_time()
+    for _ in range(reps):
+        fn()
+    return (time.process_time() - t0) / reps
+
+
+def event_ms(fn, iters=20):
+    for _ in range(3):
+        fn()
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    ev[0].record()
+    for _ in range(iters):
+        fn()
+    ev[1].record()
+    torch.cuda.synchronize()
+    return ev[0].elapsed_time(ev[1]) / iters
+
+
+def decode_leg(R, bs, reps, chunks):
+    from concurrent.futures import ThreadPoolExecutor
+    from gif_b200 import image_decode as I
+    from gif_b200.data import DeviceBatchLoader, GifLmdbDataset
+    from gif_b200.synth_images import build_lmdbs
+    with tempfile.TemporaryDirectory() as tmp:
+        real, rend = build_lmdbs(tmp, bs, R, 256)
+        ds = GifLmdbDataset(real, rend, np.zeros((bs, 8), np.float32), resolution=R, rend_flm_res=256)
+        ids = list(range(bs))
+        pil = cpu_per_batch(lambda: [ds[i] for i in ids], reps)
+        loader = DeviceBatchLoader(ds, bs)
+        with ThreadPoolExecutor(loader.threads) as pool:
+            dev_host = cpu_per_batch(lambda: loader._host_batch(ids, pool), reps)
+            hb = loader._host_batch(ids, pool)
+        row = {"resolution": R, "batch": bs, "pil_cpu_s": pil, "device_loader_host_cpu_s": dev_host,
+               "host_cpu_ratio": pil / dev_host}
+        if not torch.cuda.is_available():
+            return row
+        arena, offs, jb, pb = hb[:4]
+        d = arena.cuda()
+        seg = lambda i: d[int(offs[i]):int(offs[i + 1])]
+        out = torch.empty(jb.out_bytes, dtype=torch.uint8, device="cuda")
+        st = torch.zeros(3 * bs, dtype=torch.int32, device="cuda")
+        parsed = [I.parse_jpeg(ds.real.get(k)) for k in hb[6]]
+        ref = None
+        for cb in chunks:
+            b = I.JpegBatch(parsed, cb)
+            ints = torch.from_numpy(b.ints).cuda()
+            ws = torch.empty(b.workspace_bytes, dtype=torch.uint8, device="cuda")
+            row[f"jpeg_ms_chunk{cb}"] = event_ms(lambda: b.launch(seg(0), ints, out, st[:bs], ws))
+            ref = out.clone() if ref is None else ref
+            assert torch.equal(out, ref) and (st.cpu() == 0).all(), cb     # every chunk size decodes the same bits
+        rend_u8 = torch.empty(2 * bs, 256, 256, 3, dtype=torch.uint8, device="cuda")
+        work = seg(1).clone()
+        row["png_ms"] = event_ms(lambda: (work.copy_(seg(1)), pb.launch(work, seg(3), rend_u8, st[bs:])))
+        if R != 256:
+            row["resize_ms"] = event_ms(lambda: I.resize_bicubic_u8(rend_u8, R))
+        row["jpeg_entropy_bytes"], row["png_inflated_bytes"] = len(jb.data), pb.data_bytes
+        return row
+
+
+def trainer_leg(runs, steps, R=256, B=32, vocab=1000):
+    from gif_b200 import ops
+    from gif_b200.data import DeviceBatchLoader, GifLmdbDataset
+    from gif_b200.synth_images import build_lmdbs
+    from gif_b200.train_step import GifTrainer
+    dev = torch.device("cuda")
+    ops.set_precision("bf16x3")
+    trainer = GifTrainer(dev, R, vocab, r1_every=16, ppl=False, seed=0)
+    gen = torch.Generator().manual_seed(1234)
+    host = [(torch.rand(B, 3, R, R, generator=gen).mul_(2).sub_(1).pin_memory(),
+             torch.rand(B, 6, R, R, generator=gen).mul_(2).sub_(1).pin_memory(),
+             torch.randint(0, vocab, (B,), generator=gen).pin_memory()) for _ in range(4)]
+    trainer.iteration = 16 - 3
+    for s in range(3):
+        trainer.train_iteration(*(t.to(dev) for t in host[s]))
+    torch.cuda.synchronize()
+    trainer.capture(B, R)
+    trainer.iteration = 14
+    for s in range(2):
+        trainer.train_iteration(*host[s])
+    torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as tmp:
+        real, rend = build_lmdbs(tmp, 4 * B, R, 256)
+        ds = GifLmdbDataset(real, rend, np.zeros((4 * B, 8), np.float32), resolution=R, rend_flm_res=256)
+        loader = DeviceBatchLoader(ds, B)
+        batches = itertools.chain.from_iterable(iter(loader) for _ in itertools.count())
+        first = next(batches)
+
+        def pinned():
+            for s in range(steps):
+                trainer.train_iteration(*host[s % 4])
+
+        def device():
+            nonlocal first
+            for s in range(steps):
+                real_b, cond_b, _, idx_b = first if s == 0 else next(batches)
+                trainer.train_iteration(real_b, cond_b, idx_b)
+            first = next(batches)
+
+        res = {"pinned": [], "device_loader": []}
+        for _ in range(runs):
+            for name, fn in (("pinned", pinned), ("device_loader", device)):
+                trainer.iteration = 0                  # one R1 iteration in every window of 16
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                res[name].append(B * steps / (time.perf_counter() - t0))
+        return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--configs", default="256:32,512:16,1024:8")
+    ap.add_argument("--chunks", default="512,1024,2048,4096")
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--trainer", action="store_true")
+    ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=16)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    torch.set_num_threads(1)
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True).stdout.strip() if torch.cuda.is_available() else "no GPU"
+    res = {"card": card, "configs": []}
+    for cfg in args.configs.split(","):
+        R, bs = map(int, cfg.split(":"))
+        row = decode_leg(R, bs, args.reps, [int(c) for c in args.chunks.split(",")])
+        res["configs"].append(row)
+        print(json.dumps(row), flush=True)
+    if args.trainer:
+        res["trainer_images_per_s"] = trainer_leg(args.runs, args.steps)
+        print(json.dumps(res["trainer_images_per_s"]), flush=True)
+    res["card_after"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm", "--format=csv,noheader"],
+                                       capture_output=True, text=True).stdout.strip() if torch.cuda.is_available() else ""
+    print("card:", card, "| after:", res["card_after"])
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
