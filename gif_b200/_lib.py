@@ -58,10 +58,12 @@ SIGNATURES = {
     "gifb200_rasterize_fwd": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _sz, _p]),
     "gifb200_rasterize_fwd_ex": (_i, [_p] * 7 + [_i] * 5 + [_p, _sz, _p]),
     "gifb200_rasterize_bwd_ex": (_i, [_p] * 11 + [_i] * 5 + [_p]),
-    "gifb200_render_shade": (_i, [_p] * 9 + [_i] * 5 + [_p]),
+    "gifb200_render_shade": (_i, [_p] * 10 + [_i] * 5 + [_p]),
+    "gifb200_vertex_normals": (_i, [_p] * 6 + [_i] * 3 + [_p]),
     "gifb200_rasterize_bwd": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "gifb200_flame_lbs_workspace_bytes": (_sz, [_i, _i]),
     "gifb200_flame_lbs": (_i, [_p] * 11 + [_i] * 4 + [_p, _sz, _p]),
+    "gifb200_flametex": (_i, [_p] * 4 + [_i] * 4 + [_p]),
     "gifb200_texture_steal_fwd": (_i, [_p] * 9 + [_i] * 6 + [_p]),
     "gifb200_texture_steal_bwd": (_i, [_p] * 7 + [_i] * 6 + [_p]),
     "gifb200_jpeg_workspace_bytes": (_sz, [_i, _i, _ll]),

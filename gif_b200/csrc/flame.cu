@@ -196,3 +196,86 @@ extern "C" int gifb200_flame_lbs(const float* betas, const float* pose, const fl
     GIFB200_LAUNCH_CHECK("flame_skin_kernel");
     return GIFB200_OK;
 }
+
+// ------------------------------------------------------------------------------------------------------------ FLAMETex
+// FLAMETex.forward (models/FLAME.py:237-242): mean + basis . texcode, reshaped to side x side x 3, F.interpolate to T x T in
+// the default nearest mode (source index min(floor(dst * side / T), side - 1)), RGB -> BGR -- evaluated only at the texels
+// the nearest sampling keeps (a quarter of the basis at side 512, T 256).  One CTA per (64 output texels of one row): it
+// stages the 192 basis rows of its texels in shared memory once and runs every texcode of the batch against them, 32 at a
+// time (coefficient-major, read as float4 broadcasts), so the basis is read from HBM once per batch.
+// Algorithmic bytes per call: T*T*3*(n+1)*4 of basis + mean (39 MB at n 50, T 256) + B*n*4 + B*3*T*T*4 out.
+constexpr int kTexX = 64;
+constexpr int kTexBC = 32;
+constexpr int kTexMaxN = 200;
+
+__global__ void __launch_bounds__(kTexX * 3) flametex_kernel(const float* __restrict__ texcode, const float* __restrict__ mean,
+                                                             const float* __restrict__ basis, float* __restrict__ albedo,
+                                                             int B, int n, int side, int T, float scale) {
+    extern __shared__ __align__(16) float tex_smem[];
+    float* sB = tex_smem;                          // (kTexX*3, n): basis rows of this CTA's texels, texel-major
+    float* sT = tex_smem + kTexX * 3 * n;          // (n, kTexBC): texcodes, coefficient-major
+    const int y = blockIdx.y, x0 = blockIdx.x * kTexX, tid = threadIdx.x;
+    const int nx = min(kTexX, T - x0);
+    const int sy = min(static_cast<int>(floorf(static_cast<float>(y) * scale)), side - 1);
+    const int rowlen = 3 * n;
+    for (int i = tid; i < nx * rowlen; i += blockDim.x) {
+        const int xl = i / rowlen, e = i - xl * rowlen;
+        const int sx = min(static_cast<int>(floorf(static_cast<float>(x0 + xl) * scale)), side - 1);
+        sB[i] = __ldg(basis + (static_cast<long long>(sy) * side + sx) * rowlen + e);
+    }
+    const int c = tid / kTexX, xl = tid - c * kTexX;       // consecutive threads: consecutive x of one channel plane
+    const bool active = xl < nx;
+    const int sx = min(static_cast<int>(floorf(static_cast<float>(x0 + xl) * scale)), side - 1);
+    const float m = active ? __ldg(mean + (static_cast<long long>(sy) * side + sx) * 3 + c) : 0.f;
+    const float* brow = sB + (xl * 3 + c) * n;
+    const long long plane = static_cast<long long>(T) * T;
+    float* out = albedo + (2 - c) * plane + static_cast<long long>(y) * T + x0 + xl;
+    for (int b0 = 0; b0 < B; b0 += kTexBC) {
+        const int nb = min(kTexBC, B - b0);
+        __syncthreads();                           // sB staged / the previous pass is done with sT
+        for (int i = tid; i < n * kTexBC; i += blockDim.x) {
+            const int j = i / kTexBC, bb = i - j * kTexBC;
+            sT[i] = bb < nb ? __ldg(texcode + static_cast<long long>(b0 + bb) * n + j) : 0.f;
+        }
+        __syncthreads();
+        if (!active) continue;
+        for (int g = 0; g < nb; g += 8) {
+            float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            for (int j = 0; j < n; ++j) {
+                const float bv = brow[j];
+                const float4 t0 = *reinterpret_cast<const float4*>(sT + j * kTexBC + g);
+                const float4 t1 = *reinterpret_cast<const float4*>(sT + j * kTexBC + g + 4);
+                acc[0] = fmaf(bv, t0.x, acc[0]);
+                acc[1] = fmaf(bv, t0.y, acc[1]);
+                acc[2] = fmaf(bv, t0.z, acc[2]);
+                acc[3] = fmaf(bv, t0.w, acc[3]);
+                acc[4] = fmaf(bv, t1.x, acc[4]);
+                acc[5] = fmaf(bv, t1.y, acc[5]);
+                acc[6] = fmaf(bv, t1.z, acc[6]);
+                acc[7] = fmaf(bv, t1.w, acc[7]);
+            }
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+                if (g + q < nb) out[static_cast<long long>(b0 + g + q) * 3 * plane] = m + acc[q];
+        }
+    }
+}
+
+extern "C" int gifb200_flametex(const float* texcode, const float* mean, const float* basis, float* albedo, int B, int n,
+                                int side, int T, gifb200_stream_t stream) {
+    GIFB200_REQUIRE(B >= 0 && n >= 1 && n <= kTexMaxN && side > 0 && T > 0 && T <= 65535, GIFB200_E_SHAPE,
+                    "flametex: bad shape (1 <= n <= 200 coefficients, T <= 65535)");
+    if (B == 0) return GIFB200_OK;
+    const int smem = static_cast<int>(sizeof(float)) * (kTexX * 3 + kTexBC) * n;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(flametex_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             static_cast<int>(sizeof(float)) * (kTexX * 3 + kTexBC) * kTexMaxN);
+        if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "flametex smem attribute", cudaGetErrorString(e));
+        attr = true;
+    }
+    flametex_kernel<<<dim3(cdiv(T, kTexX), T), kTexX * 3, smem, static_cast<cudaStream_t>(stream)>>>(
+        texcode, mean, basis, albedo, B, n, side, T, static_cast<float>(side) / static_cast<float>(T));
+    GIFB200_LAUNCH_CHECK("flametex_kernel");
+    return GIFB200_OK;
+}

@@ -292,12 +292,15 @@ def decode_image(data, resolution=None):
 
 class GifLmdbDataset(torch.utils.data.Dataset):
     """The reference's FFHQ item for ``rendered_flame_as_condition=True, normal_maps_as_cond=True`` (dataset_loaders.py:236-330):
-    ``(img (3,R,R), [cond (6,R,R)], [flame_label (P,)], index)``, all float32, images in [-1,1]."""
+    ``(img (3,R,R), [cond (6,R,R)], [flame_label (P,)], index)``, all float32, images in [-1,1].
+
+    ``rendered_flame_root=None``: there is no render LMDB; the conditions are rendered on the device from the raw parameter
+    rows by ``DeviceBatchLoader(dataset, ..., conditions=DecaConditionRenderer(...))``, and indexing the dataset raises."""
 
     def __init__(self, real_img_root, rendered_flame_root, flame_params, resolution=256, rend_flm_res=256, valid_ids=None,
                  flame_mean=0.0, flame_std=1.0):
         self.real = LmdbReader(real_img_root)
-        self.rend = LmdbReader(rendered_flame_root)
+        self.rend = None if rendered_flame_root is None else LmdbReader(rendered_flame_root)
         self.length = int(self.real.get(b"length").decode("utf-8"))           # dataset_loaders.py:168
         self.resolution, self.rend_flm_res = resolution, rend_flm_res
         self.flame_params = np.asarray(flame_params, dtype=np.float32)
@@ -308,6 +311,9 @@ class GifLmdbDataset(torch.utils.data.Dataset):
         return len(self.valid_ids)
 
     def __getitem__(self, index):
+        if self.rend is None:
+            raise RuntimeError("this dataset has no render LMDB (rendered_flame_root=None): its conditions are rendered on the "
+                               "device, so batches come from DeviceBatchLoader(dataset, ..., conditions=DecaConditionRenderer(...))")
         i = int(self.valid_ids[index])
         img = decode_image(self.real.get(image_key(self.resolution, i)))
         rnd = decode_image(self.rend.get(image_key(self.rend_flm_res, i)), self.resolution)
@@ -371,12 +377,26 @@ class DeviceBatchLoader:
     cond (B,6,R,R), labels (B,P), indices (B,) int64) -- the arguments of ``GifTrainer.train_iteration`` -- after making the
     current stream wait for their decode.  Each batch stays valid until the next one is requested.  Before yielding a batch
     it waits for that batch's decode (queued a step earlier on the side stream, never behind training work) and reads its
-    per-image status words, so a corrupt image raises before its batch is used."""
+    per-image status words, so a corrupt image raises before its batch is used.
 
-    def __init__(self, dataset, batch_size, shuffle=True, seed=0, depth=3, device=None, threads=4):
+    ``conditions``: a ``gif_b200.conditions.DecaConditionRenderer`` at the dataset's ``rend_flm_res``.  The conditions are
+    then rendered on the side stream from the raw parameter rows (``dataset.flame_params``), which travel with the labels;
+    no render key is read and nothing is inflated.  The rendered bytes are what the reference's render LMDB holds, so the
+    batches equal those of the LMDB path wherever the rasteriser agrees with the one that wrote it."""
+
+    def __init__(self, dataset, batch_size, shuffle=True, seed=0, depth=3, device=None, threads=4, conditions=None):
         self.ds, self.bs, self.shuffle, self.seed, self.depth = dataset, batch_size, shuffle, seed, depth
         self.device = torch.device(device or "cuda")
         self.threads = threads
+        if conditions is not None and conditions.image_size != dataset.rend_flm_res:
+            raise ValueError(f"the condition renderer draws {conditions.image_size}^2, the dataset's rend_flm_res is "
+                             f"{dataset.rend_flm_res}")
+        if conditions is not None and dataset.flame_params.shape[-1] < 236:
+            raise ValueError(f"rendering conditions needs DECA rows of at least 236 columns, the dataset's parameter table "
+                             f"has {dataset.flame_params.shape[-1]}")
+        if conditions is None and dataset.rend is None:
+            raise ValueError("the dataset has no render LMDB (rendered_flame_root=None): pass conditions=DecaConditionRenderer(...)")
+        self.conditions = conditions
         self.pin = torch.cuda.is_available()
         self._stream = None
 
@@ -384,7 +404,8 @@ class DeviceBatchLoader:
         from . import image_decode as I
         ds, R, rr = self.ds, self.ds.resolution, self.ds.rend_flm_res
         keys = [image_key(R, i) for i in ids]
-        rkeys = [image_key(rr, i) for i in ids] + [normal_map_key(rr, i) for i in ids]
+        render = self.conditions is not None
+        rkeys = [] if render else [image_key(rr, i) for i in ids] + [normal_map_key(rr, i) for i in ids]
 
         def png(k):
             try:
@@ -394,7 +415,7 @@ class DeviceBatchLoader:
                 return h, I.inflate_png(h)
             except I.UnsupportedImage as e:
                 raise I.UnsupportedImage(f"{k.decode()}: {e}") from None
-        pngs = pool.map(png, rkeys)                 # inflates on the pool while this thread parses the JPEGs
+        pngs = pool.map(png, rkeys)                 # inflates on the pool while this thread parses the JPEGs (if any)
         parsed = []
         for k in keys:
             try:
@@ -406,8 +427,8 @@ class DeviceBatchLoader:
             parsed.append(p)
         pngs = list(pngs)
         jb = I.JpegBatch(parsed)
-        pb = I.PngBatch([h for h, _ in pngs], [r for _, r in pngs])
-        sizes = [len(jb.data), pb.data_bytes, 4 * jb.ints.size, 4 * pb.desc.size]
+        pb = None if render else I.PngBatch([h for h, _ in pngs], [r for _, r in pngs])
+        sizes = [len(jb.data), 0 if render else pb.data_bytes, 4 * jb.ints.size, 0 if render else 4 * pb.desc.size]
         offs = np.concatenate([[0], np.cumsum([(s + 255) // 256 * 256 for s in sizes])])
         arena = torch.empty(int(offs[-1]), dtype=torch.uint8, pin_memory=self.pin)
         a = arena.numpy()
@@ -417,15 +438,18 @@ class DeviceBatchLoader:
             a[o:o + len(r)] = np.frombuffer(r, np.uint8)
             o += len(r)
         a[offs[2]:offs[2] + sizes[2]] = jb.ints.view(np.uint8)
-        a[offs[3]:offs[3] + sizes[3]] = pb.desc.ravel().view(np.uint8)
+        if not render:
+            a[offs[3]:offs[3] + sizes[3]] = pb.desc.ravel().view(np.uint8)
         lbl = np.stack([(ds.flame_params[i] - ds.flame_mean) / ds.flame_std for i in ids]).astype(np.float32)
         pin = (lambda t: t.pin_memory()) if self.pin else (lambda t: t)
-        return arena, offs, jb, pb, pin(torch.from_numpy(lbl)), pin(torch.tensor(ids, dtype=torch.int64)), keys, rkeys
+        # the renderer takes the raw rows: (p - m) / s * s + m is not p in float32
+        raw = pin(torch.from_numpy(np.ascontiguousarray(ds.flame_params[ids], dtype=np.float32))) if render else None
+        return arena, offs, jb, pb, pin(torch.from_numpy(lbl)), pin(torch.tensor(ids, dtype=torch.int64)), raw, keys, rkeys
 
     def _launch(self, hb):
         """Enqueue the copy and the decode of one host batch on the side stream."""
         from . import image_decode as I
-        arena, offs, jb, pb, lbl, idx, keys, rkeys = hb
+        arena, offs, jb, pb, lbl, idx, raw, keys, rkeys = hb
         dev, B, R, rr = self.device, self.bs, self.ds.resolution, self.ds.rend_flm_res
         with torch.cuda.stream(self._stream):
             d = arena.to(dev, non_blocking=True)
@@ -435,7 +459,10 @@ class DeviceBatchLoader:
             rend_u8 = torch.empty(2 * B, rr, rr, 3, dtype=torch.uint8, device=dev)
             ws = torch.empty(jb.workspace_bytes, dtype=torch.uint8, device=dev)
             jb.launch(seg(0), seg(2), real_u8, status[:B], ws)
-            pb.launch(seg(1), seg(3), rend_u8, status[B:])
+            if raw is None:
+                pb.launch(seg(1), seg(3), rend_u8, status[B:])
+            else:
+                self.conditions.render_u8(raw.to(dev, non_blocking=True), out=rend_u8)
             if rr != R:
                 rend_u8 = I.resize_bicubic_u8(rend_u8, R)
             real = torch.empty(B, 3, R, R, device=dev)

@@ -12,7 +12,6 @@ import pickle
 import numpy as np
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from . import ops
 from ._lib import check, lib, ptr, require_cuda, stream
@@ -170,8 +169,11 @@ class FLAME(nn.Module):
 
 
 class FLAMETex(nn.Module):
-    """FLAME.py:220-244: linear texture space (BFM-derived), texcode (B,n) -> albedo (B,3,256,256) RGB in 0..255.
-    The basis product runs through ``gifb200_sgemm`` (memory-bound on the (512*512*3, n) basis)."""
+    """FLAME.py:220-244: linear texture space (BFM-derived), texcode (B,n) -> albedo (B,3,256,256), BGR, in the units of
+    the texture space (0..255 for FLAME_texture.npz).  ``gifb200_flametex`` evaluates the basis only at the texels the
+    reference's nearest resize to 256 keeps, reading that part of the basis once per batch."""
+
+    SIZE = 256
 
     def __init__(self, config=None, mean=None, basis=None):
         super().__init__()
@@ -183,9 +185,15 @@ class FLAMETex(nn.Module):
 
     @torch.no_grad()
     def forward(self, texcode):
-        B = texcode.shape[0]
-        side = int(round((self.texture_mean.shape[-1] // 3) ** 0.5))
-        tex = self.texture_mean.reshape(1, -1) + ops.matmul(texcode.float().contiguous(), self.texture_basis[0], trans_b=True)
-        tex = tex.reshape(B, side, side, 3).permute(0, 3, 1, 2)
-        tex = F.interpolate(tex, [256, 256])
-        return tex[:, [2, 1, 0], :, :]
+        texcode = texcode.float().contiguous()
+        require_cuda(texcode, self.texture_basis)
+        B, n = texcode.shape
+        K = self.texture_mean.shape[-1]
+        side = int(round((K // 3) ** 0.5))
+        if side * side * 3 != K or self.texture_basis.shape[1:] != (K, n):
+            raise ValueError(f"FLAMETex: texcode ({B}, {n}) does not match the texture space (mean {K}, basis "
+                             f"{tuple(self.texture_basis.shape[1:])}, a square RGB texture)")
+        out = torch.empty(B, 3, self.SIZE, self.SIZE, device=texcode.device)
+        check(lib.gifb200_flametex(ptr(texcode), ptr(self.texture_mean), ptr(self.texture_basis), ptr(out), B, n, side,
+                                   self.SIZE, stream()), "gifb200_flametex")
+        return out

@@ -174,3 +174,43 @@ def synthetic_texture_data(size=256):
             "valid_pixel_b_coords": bary.reshape(-1, 3)[valid].astype(np.float32)}
     _cache[("tex", size)] = data
     return data
+
+
+def synthetic_texture_space(side=512, n=50):
+    """A FLAMETex-shaped texture space (the licence-gated FLAME_texture.npz is absent), defined analytically so that it can
+    be rebuilt anywhere instead of stored: texel (x, y), channel c, k = (y*side + x)*3 + c, u = x/side, v = y/side,
+        mean[k]     = 128 + 60 cos(2 pi (1.5 u + 0.5 v) + 0.9 c)
+        tex_dir[k,j] = 12 / (1 + 0.1 j) * cos(2 pi ((1 + j mod 5) u + (1 + 3j mod 7) v) + 0.37 j + (1.3 + 0.11 j) c)
+    evaluated in float64 and rounded to float32.  -> (mean (side*side*3,), tex_dir (side*side*3, n)) numpy float32."""
+    k = np.arange(side * side * 3, dtype=np.int64)
+    c = (k % 3).astype(np.float64)
+    u = ((k // 3) % side).astype(np.float64) / side
+    v = (k // (3 * side)).astype(np.float64) / side
+    mean = (128.0 + 60.0 * np.cos(2 * np.pi * (1.5 * u + 0.5 * v) + 0.9 * c)).astype(np.float32)
+    tex_dir = np.empty((k.size, n), np.float32)
+    for j in range(n):
+        arg = 2 * np.pi * ((1 + j % 5) * u + (1 + (3 * j) % 7) * v) + 0.37 * j + (1.3 + 0.11 * j) * c
+        tex_dir[:, j] = 12.0 / (1.0 + 0.1 * j) * np.cos(arg)
+    return mean, tex_dir
+
+
+def synthetic_deca_params(n, seed=0, cols=236):
+    """(n, cols) DECA parameter rows [shape 100 | exp 50 | pose 6 | cam 3 | tex 50 | lit 27 | extra] in realistic ranges for
+    the synthetic model: cam scale 7-10, yaw within +-pi/8, lights as ``synthetic_flame_params``."""
+    g = torch.Generator().manual_seed(seed)
+    p = torch.zeros(n, cols)
+    p[:, 0:100] = torch.randn(n, 100, generator=g)
+    p[:, 100:150] = torch.randn(n, 50, generator=g) * 0.5
+    p[:, 150] = torch.rand(n, generator=g) * 0.2 - 0.1                          # pitch
+    p[:, 151] = (torch.rand(n, generator=g) * 2 - 1) * (math.pi / 8)           # yaw
+    p[:, 153] = torch.rand(n, generator=g) * 0.2                                # jaw
+    p[:, 156] = torch.rand(n, generator=g) * 3 + 7
+    p[:, 157:159] = (torch.rand(n, 2, generator=g) * 2 - 1) * 0.02
+    p[:, 159:209] = torch.randn(n, 50, generator=g)
+    lit = torch.zeros(n, 9, 3)
+    lit[:, 0] = 3.0 + 0.3 * torch.randn(n, 3, generator=g)
+    lit[:, 1:] = 0.3 * torch.randn(n, 8, 3, generator=g)
+    p[:, 209:236] = lit.reshape(n, 27)
+    if cols > 236:
+        p[:, 236:] = torch.randn(n, cols - 236, generator=g)
+    return p

@@ -11,7 +11,7 @@ import torch.nn as nn
 
 from . import ops
 from ._lib import check, lib, ptr, require_cuda, stream
-from .render import batch_orth_proj, vertex_normals
+from .render import batch_orth_proj, vertex_adjacency, vertex_normals
 
 
 class _TextureSteal(torch.autograd.Function):
@@ -89,6 +89,7 @@ class FlameTextureSpace(nn.Module):
         self.flame = flame
         self.size = size
         self._table = None
+        self._adj = None
 
     @staticmethod
     def _flame_from_constants():
@@ -119,7 +120,9 @@ class FlameTextureSpace(nn.Module):
             verts, _ = self.flame.decode_vertices(shape, exp, pose)
             trans = batch_orth_proj(verts, cam)
             trans[:, :, 1:] = -trans[:, :, 1:]
-            normals = vertex_normals(trans, self.flame.faces_tensor)
+            if self._adj is None or self._adj[0].device != trans.device:
+                self._adj = vertex_adjacency(self.flame.faces_tensor.to(trans.device), trans.shape[1])
+            normals = vertex_normals(trans, self.flame.faces_tensor, self._adj)
         return self.compute_texture_map(source_img, verts, normals, camera_params=cam)
 
     def compute_texture_map(self, source_img, target_mesh_v, vertex_normals, camera_params):

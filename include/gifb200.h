@@ -280,15 +280,25 @@ int gifb200_rasterize_bwd_ex(const float* face_vertices, const float* face_color
 
 /* Fused shading epilogue of the FLAME conditioning render: from the rasteriser's (triangle, bary) buffers to the textured
  * image tex (B,h,w,3) = albedo(uv) * SH-shading(normal) * alpha, the normal image nrm (B,h,w,3), and the quantised
- * 6-channel condition map cond (B,h,w,6) in [-1,1] (each output may be NULL).
+ * 6-channel condition map cond (B,h,w,6) in [-1,1], and cond_u8 (2B,h,w,3) uint8: planes 0..B-1 floor(clamp(tex,0,255)),
+ * planes B..2B-1 floor(clamp(nrm,0,1)*255) -- the bytes prepare_lmdb/create_deca_rendered_lmdb.py stores in its PNGs, in
+ * the layout of gifb200_png_unfilter's output (each output may be NULL).
  * Replaces the attribute interpolation of Pytorch3dRasterizer.forward (photometric_optimization/renderer.py:69-84),
  * Renderer.forward's grid_sample / add_SHlight / composition (renderer.py:152-221), Renderer.render_normal (:291-305),
  * OverLayViz.get_rendered_mesh's quantisation (my_utils/visualize_flame_overlay.py:29-31) and the consumer's mapping
  * to [-1,1] (loss_functions/losses.py:213-214).  face_uv (F,3,2) grid coordinates in [-1,1] (shared by the batch),
  * face_normals (B,F,3,3) world-space vertex normals per face corner, albedo (B,3,T,T), sh (B,9,3). */
 int gifb200_render_shade(const int32_t* triangle, const float* bary, const float* face_uv, const float* face_normals,
-                         const float* albedo, const float* sh, float* tex, float* nrm, float* cond, int B, int F, int h,
-                         int w, int T, gifb200_stream_t stream);
+                         const float* albedo, const float* sh, float* tex, float* nrm, float* cond, uint8_t* cond_u8, int B,
+                         int F, int h, int w, int T, gifb200_stream_t stream);
+
+/* Area-weighted vertex normals, util.vertex_normals (my_utils/photometric_optimization/util.py:156-189), deterministic:
+ * every vertex sums its face corners' cross products in the order of a CSR adjacency built once per topology --
+ * adj_offsets (V+1), adj_corners (3F) = f*3 + corner, ascending per vertex -- then divides by max(|n|, 1e-6).
+ * verts (B,V,3), faces (F,3) int32.  Outputs (each may be NULL): normals (B,V,3); face_normals (B,F,3,3), the normal of
+ * every face corner's vertex (what gifb200_render_shade reads). */
+int gifb200_vertex_normals(const float* verts, const int32_t* faces, const int32_t* adj_offsets, const int32_t* adj_corners,
+                           float* normals, float* face_normals, int B, int V, int F, gifb200_stream_t stream);
 
 /* FLAME decoder: linear blend skinning, lbs() of my_utils/photometric_optimization/models/lbs.py:141-228 as called by
  * FLAME.forward (models/FLAME.py:175-216).  betas (B,NB) = [shape | expression], pose (B,NJ*3) axis-angle per joint
@@ -303,6 +313,13 @@ int gifb200_flame_lbs(const float* betas, const float* pose, const float* v_temp
                       const float* posedirs, const float* j_template, const float* j_shapedirs, const int32_t* parents,
                       const float* lbs_weights, float* verts, float* joints, int B, int V, int NB, int NJ, void* ws,
                       size_t ws_bytes, gifb200_stream_t stream);
+
+/* FLAMETex.forward (models/FLAME.py:237-242) at the texels its nearest resize keeps: albedo (B,3,T,T) BGR,
+ * albedo[b,2-c,y,x] = mean[k] + sum_j basis[k,j] texcode[b,j] with k = (sy*side + sx)*3 + c, sy = min(floor(y*side/T),
+ * side-1) (likewise sx) in float32 as F.interpolate's nearest mode computes it.  texcode (B,n), mean (side*side*3),
+ * basis (side*side*3, n) row-major (the reference's texture_basis[0]); 1 <= n <= 200. */
+int gifb200_flametex(const float* texcode, const float* mean, const float* basis, float* albedo, int B, int n, int side, int T,
+                     gifb200_stream_t stream);
 
 /* Texture stealing, FlameTextureSpace.compute_texture_map (model/stg2_generator.py:376-421): for every texel of the T x T
  * FLAME UV atlas, bilinear sample (zeros padding, align_corners = False) of the image src (B,H,W,C) channels-last at the

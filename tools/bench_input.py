@@ -8,6 +8,9 @@
    the bytes each pass reads.
 3. ``--trainer``: GifTrainer images/s at 256^2 batch 32 (bf16x3, CUDA graphs, no path-length term) fed by DeviceBatchLoader
    against the same step fed from pinned host tensors, alternating, three runs of each.
+4. ``--conditions render``: the same legs with the conditions rendered on the device from DECA rows
+   (DeviceBatchLoader(conditions=DecaConditionRenderer), synthetic FLAME model, analytic 512^2 x 50 texture space) next to
+   the PNG path: host CPU s/batch, device ms/batch of the render against the PNG unfilter, and a third trainer arm.
 
 The synthetic LMDBs follow the reference's writers (JPEG q100 4:2:0 real images, PNG renders at 256^2).  Prints the card,
 its power limit and clocks read in the same run; writes JSON to --out."""
@@ -46,7 +49,34 @@ def event_ms(fn, iters=20):
     return ev[0].elapsed_time(ev[1]) / iters
 
 
-def decode_leg(R, bs, reps, chunks):
+def condition_renderer(rr):
+    from gif_b200.conditions import DecaConditionRenderer
+    from gif_b200.flame import FLAME, FLAMETex
+    from gif_b200.flame_synth import flame_uv, synthetic_flame_model, synthetic_texture_space
+    mean, basis = synthetic_texture_space(512, 50)
+    return DecaConditionRenderer(FLAME.from_arrays(synthetic_flame_model()).cuda(), FLAMETex(mean=mean, basis=basis).cuda(),
+                                 *flame_uv(), image_size=rr)
+
+
+def render_leg(row, real, R, bs, reps, cr):
+    """Host CPU s/batch of the render-fed loader and device ms/batch of the render (FLAME, FLAMETex, rasteriser, shading)."""
+    from concurrent.futures import ThreadPoolExecutor
+    from gif_b200.data import DeviceBatchLoader, GifLmdbDataset
+    from gif_b200.flame_synth import synthetic_deca_params
+    params = synthetic_deca_params(bs, 3).numpy()
+    ds = GifLmdbDataset(real, None, params, resolution=R, rend_flm_res=256)
+    loader = DeviceBatchLoader(ds, bs, conditions=cr)
+    ids = list(range(bs))
+    with ThreadPoolExecutor(loader.threads) as pool:
+        row["render_loader_host_cpu_s"] = cpu_per_batch(lambda: loader._host_batch(ids, pool), reps)
+    raw = torch.from_numpy(params).cuda()
+    out = torch.empty(2 * bs, 256, 256, 3, dtype=torch.uint8, device="cuda")
+    row["render_ms"] = event_ms(lambda: cr.render_u8(raw, out=out))
+    row["flametex_ms"] = event_ms(lambda: cr.flametex(raw[:, 159:209]))
+    row["flametex_bytes"] = 256 * 256 * 3 * 51 * 4 + bs * 3 * 256 * 256 * 4
+
+
+def decode_leg(R, bs, reps, chunks, cr=None):
     from concurrent.futures import ThreadPoolExecutor
     from gif_b200 import image_decode as I
     from gif_b200.data import DeviceBatchLoader, GifLmdbDataset
@@ -69,7 +99,7 @@ def decode_leg(R, bs, reps, chunks):
         seg = lambda i: d[int(offs[i]):int(offs[i + 1])]
         out = torch.empty(jb.out_bytes, dtype=torch.uint8, device="cuda")
         st = torch.zeros(3 * bs, dtype=torch.int32, device="cuda")
-        parsed = [I.parse_jpeg(ds.real.get(k)) for k in hb[6]]
+        parsed = [I.parse_jpeg(ds.real.get(k)) for k in hb[7]]
         ref = None
         for cb in chunks:
             b = I.JpegBatch(parsed, cb)
@@ -84,10 +114,12 @@ def decode_leg(R, bs, reps, chunks):
         if R != 256:
             row["resize_ms"] = event_ms(lambda: I.resize_bicubic_u8(rend_u8, R))
         row["jpeg_entropy_bytes"], row["png_inflated_bytes"] = len(jb.data), pb.data_bytes
+        if cr is not None:
+            render_leg(row, real, R, bs, reps, cr)
         return row
 
 
-def trainer_leg(runs, steps, R=256, B=32, vocab=1000):
+def trainer_leg(runs, steps, R=256, B=32, vocab=1000, cr=None):
     from gif_b200 import ops
     from gif_b200.data import DeviceBatchLoader, GifLmdbDataset
     from gif_b200.synth_images import build_lmdbs
@@ -114,21 +146,31 @@ def trainer_leg(runs, steps, R=256, B=32, vocab=1000):
         loader = DeviceBatchLoader(ds, B)
         batches = itertools.chain.from_iterable(iter(loader) for _ in itertools.count())
         first = next(batches)
+        arms = {"pinned": None, "device_loader": [batches, first]}
+        if cr is not None:
+            from gif_b200.flame_synth import synthetic_deca_params
+            rds = GifLmdbDataset(real, None, synthetic_deca_params(4 * B, 5).numpy(), resolution=R, rend_flm_res=256)
+            rloader = DeviceBatchLoader(rds, B, conditions=cr)
+            rb = itertools.chain.from_iterable(iter(rloader) for _ in itertools.count())
+            arms["render_loader"] = [rb, next(rb)]
 
         def pinned():
             for s in range(steps):
                 trainer.train_iteration(*host[s % 4])
 
-        def device():
-            nonlocal first
-            for s in range(steps):
-                real_b, cond_b, _, idx_b = first if s == 0 else next(batches)
-                trainer.train_iteration(real_b, cond_b, idx_b)
-            first = next(batches)
+        def fed(arm):
+            def run():
+                src, first = arm
+                for s in range(steps):
+                    real_b, cond_b, _, idx_b = first if s == 0 else next(src)
+                    trainer.train_iteration(real_b, cond_b, idx_b)
+                arm[1] = next(src)
+            return run
 
-        res = {"pinned": [], "device_loader": []}
+        fns = [(name, pinned if arm is None else fed(arm)) for name, arm in arms.items()]
+        res = {name: [] for name in arms}
         for _ in range(runs):
-            for name, fn in (("pinned", pinned), ("device_loader", device)):
+            for name, fn in fns:
                 trainer.iteration = 0                  # one R1 iteration in every window of 16
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
@@ -146,19 +188,22 @@ def main():
     ap.add_argument("--trainer", action="store_true")
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--steps", type=int, default=16)
+    ap.add_argument("--conditions", choices=("lmdb", "render"), default="lmdb",
+                    help="render: also measure conditions rendered on the device from DECA rows")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     torch.set_num_threads(1)
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip() if torch.cuda.is_available() else "no GPU"
     res = {"card": card, "configs": []}
+    cr = condition_renderer(256) if args.conditions == "render" else None
     for cfg in args.configs.split(","):
         R, bs = map(int, cfg.split(":"))
-        row = decode_leg(R, bs, args.reps, [int(c) for c in args.chunks.split(",")])
+        row = decode_leg(R, bs, args.reps, [int(c) for c in args.chunks.split(",")], cr)
         res["configs"].append(row)
         print(json.dumps(row), flush=True)
     if args.trainer:
-        res["trainer_images_per_s"] = trainer_leg(args.runs, args.steps)
+        res["trainer_images_per_s"] = trainer_leg(args.runs, args.steps, cr=cr)
         print(json.dumps(res["trainer_images_per_s"]), flush=True)
     res["card_after"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm", "--format=csv,noheader"],
                                        capture_output=True, text=True).stdout.strip() if torch.cuda.is_available() else ""
