@@ -54,13 +54,13 @@ struct WgParams {
 
 constexpr int kHaloRows = kPix + 2;                 // 34 pixel rows: the 32 of the stage + one on each side
 
-// HALO (fp32, stride-1 layers with Ws >= 32): the KW shifted big-tensor tiles of a stage overlap in all but 2 pixel rows, so
+// HALO (stride-1 3x3 layers with Ws >= 32): the KW shifted big-tensor tiles of a stage overlap in all but 2 pixel rows, so
 // the stage holds ONE (32 + 2)-row tile per 32-channel chunk and tap kw reads it from pixel row kw on.
 template <int KW, int BLOCK_N, bool HALO = false, bool X3 = false, int AC = 4>
 struct WgSmem {
     static constexpr int kRowBytes = X3 ? 64 : 128;                   // 32 channels of one pixel
     static constexpr int kChunkBytes = kPix * kRowBytes;              // one 32-channel x 32-pixel chunk: 4 KB fp32, 2 KB bf16
-    static constexpr int kHaloChunkBytes = 5120;                      // 34 rows of 128 B padded to the 1024 B swizzle atom
+    static constexpr int kHaloChunkBytes = X3 ? 2560 : 5120;          // 34 rows padded to the swizzle atom (512 B bf16, 1024 B fp32)
     static constexpr int kPlanes = X3 ? 2 : 1;                        // hi and lo chunk sets, hi first
     static constexpr int kBChunks = BLOCK_N / 32;
     static constexpr int kAPlaneBytes = AC * kChunkBytes;         // AC 32-channel A chunks: M = 32 * AC small channels
@@ -72,7 +72,6 @@ struct WgSmem {
     static constexpr int kTxBytes = HALO ? kABytes + kPlanes * kBChunks * kHaloRows * kRowBytes : kStageBytes;
     static constexpr int kBarrierOffset = (kStages * kStageBytes + 1023) / 1024 * 1024;
     static constexpr int kDynamic = kBarrierOffset + 128 + 1024;
-    static_assert(!(HALO && X3), "the halo tile is an fp32-only layout");
 };
 
 // byte offset of (pixel row, channel) in a 32-channel fp32 chunk written by TMA with SWIZZLE_128B (1024 B aligned chunk):
@@ -81,7 +80,7 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int ch) {
     return static_cast<uint32_t>(row * 128 + ((((ch >> 2) ^ row) & 7) << 4) + (ch & 3) * 4);
 }
 
-template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC>
+template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC, bool RS>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_s,
                                                                  const __grid_constant__ CUtensorMap map_s2,
                                                                  const __grid_constant__ CUtensorMap map_b,
@@ -201,25 +200,54 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
             for (int i = 0; i < kAcc; ++i) acc[kw][i] = 0.f;
         int stage = 0, prev = -1;
         uint32_t ph = 0;
-        for (int it = 0; it < iters; ++it) {
+        // RS: the A operand of a slice (this warpgroup's 64 rows x 16 pixels of S, hi and lo plane) is the same for all KW
+        // taps and for two of the three MMAs of each tap, so it is loaded into registers once per slice (ldmatrix .trans of
+        // the MN-major tile) and only B is read from shared memory by the wgmmas: half the operand bytes of SS.  The MMAs,
+        // their order and the accumulators are those of SS.  wgmma reads the fragments asynchronously and the previous
+        // stage's group is still in flight when the next stage loads its own, so the fragments alternate between two sets.
+        uint32_t afr[2][kSlices][2][4];      // [set][slice][plane: 0 = hi, 1 = lo][register]
+        // this lane's ldmatrix row: matrix mi = lane / 8 covers rows +8 (mi & 1) and pixels +8 (mi >> 1) of the warp's 16 x 16
+        // block, row r = lane % 8 is pixel r of it; a pixel row is 64 B and SWIZZLE_64B XORs its 16 B unit with (pixel / 2) % 4
+        const int mi = lane >> 3, r8 = lane & 7;
+        const uint32_t a_lane = (AC == 4 ? wg * 2 * kChunkBytes : 0) + (wq >> 1) * kChunkBytes + (8 * (mi >> 1) + r8) * 64 +
+                                ((((2 * wq + (mi & 1)) & 3) ^ (r8 >> 1)) << 4);
+        auto run_stage = [&](uint32_t (&fr)[kSlices][2][4]) {
             mbar_wait(&full_bar[stage], ph);
             const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
             const uint32_t a_row = AC == 4 ? wg * 2 * kChunkBytes : 0;
             const uint64_t adesc = make_smem_desc(a_addr + a_row, kChunkBytes, 512, 2);
             const uint64_t adesc_lo = make_smem_desc(a_addr + L::kAPlaneBytes + a_row, kChunkBytes, 512, 2);
+            if constexpr (RS) {
+#pragma unroll
+                for (int jj = 0; jj < kSlices; ++jj) {
+                    const int j = AC == 4 ? jj : wg;
+#pragma unroll
+                    for (int pl = 0; pl < 2; ++pl) ldmatrix_x4_trans(fr[jj][pl], a_addr + pl * L::kAPlaneBytes + a_lane + 1024 * j);
+                }
+            }
             wgmma_fence();
 #pragma unroll
             for (int kw = 0; kw < KW; ++kw) {
                 fence_regs<kAcc>(acc[kw]);
-                const uint32_t b_addr = a_addr + L::kABytes + kw * L::kBBytesPerTap;
-                const uint64_t bdesc = make_smem_desc(b_addr, kChunkBytes, 512, 2);
-                const uint64_t bdesc_lo = make_smem_desc(b_addr + L::kBPlaneBytes, kChunkBytes, 512, 2);
+                // HALO: tap kw starts kw pixel rows (64 B each) into the halo tile, inside a 512 B swizzle atom.  wgmma applies
+                // the SWIZZLE_64B XOR to the absolute shared-memory address, as TMA wrote it, so the descriptor simply starts
+                // there (base offset 0; the tests compare every tap bitwise with the one-tile-per-tap layout).
+                const uint32_t b_addr = a_addr + L::kABytes + (HALO ? kw * L::kRowBytes : kw * L::kBBytesPerTap);
+                const uint32_t b_lbo = HALO ? kHaloChunkBytes : kChunkBytes;
+                const uint64_t bdesc = make_smem_desc(b_addr, b_lbo, 512, 2);
+                const uint64_t bdesc_lo = make_smem_desc(b_addr + L::kBPlaneBytes, b_lbo, 512, 2);
 #pragma unroll
                 for (int jj = 0; jj < kSlices; ++jj) {   // 16 pixels per MMA = two 8-pixel atoms: next slice = +1024 B (>>4 = 64)
                     const int j = AC == 4 ? jj : wg;
-                    wgmma_bf16<BLOCK_N>(acc[kw], adesc_lo + 64 * j, bdesc + 64 * j, 1, Trans<1>());
-                    wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc_lo + 64 * j, 1, Trans<1>());
-                    wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc + 64 * j, 1, Trans<1>());
+                    if constexpr (RS) {
+                        wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][1], bdesc + 64 * j, 1, Trans<1>());
+                        wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][0], bdesc_lo + 64 * j, 1, Trans<1>());
+                        wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][0], bdesc + 64 * j, 1, Trans<1>());
+                    } else {
+                        wgmma_bf16<BLOCK_N>(acc[kw], adesc_lo + 64 * j, bdesc + 64 * j, 1, Trans<1>());
+                        wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc_lo + 64 * j, 1, Trans<1>());
+                        wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc + 64 * j, 1, Trans<1>());
+                    }
                 }
             }
             wgmma_commit();
@@ -229,6 +257,14 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
             if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
             prev = stage;
             if (++stage == kNStages) { stage = 0; ph ^= 1; }
+        };
+        if constexpr (RS) {
+            for (int it = 0; it < iters; it += 2) {
+                run_stage(afr[0]);
+                if (it + 1 < iters) run_stage(afr[1]);
+            }
+        } else {
+            for (int it = 0; it < iters; ++it) run_stage(afr[0]);
         }
         wgmma_wait<0>();
 #pragma unroll
@@ -366,17 +402,17 @@ int pick_bn(int Cb) {
 
 struct WgMaps { CUtensorMap s, s2, b, b2; };
 
-template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC>
+template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC, bool RS>
 int launch_wg(const WgMaps& m, float* out, float* part, const WgParams& p, cudaStream_t st) {
     using L = WgSmem<KW, BLOCK_N, HALO, X3, AC>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
+        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
         if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "cudaFuncSetAttribute(wgrad_tc_kernel)", cudaGetErrorString(e));
         attr_set = true;
     }
     dim3 grid(STACK || AC == 2 ? 1 : p.Cs / 128, p.Cb / BLOCK_N, STACK ? p.splits : p.k * p.splits);
-    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
+    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC, RS><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
     GIFB200_LAUNCH_CHECK("wgrad_tc_kernel");
     const int T = p.k * p.k;
     const long long total = static_cast<long long>(T) * p.Cs * p.Cb;
@@ -435,21 +471,18 @@ size_t conv2d_wgrad_tc_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, in
     return static_cast<size_t>(wgrad_splits(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, nullptr)) * k * k * Co * Ci * sizeof(float) + 256;
 }
 
-template <bool X3>
+template <bool X3, bool RS>
 static int dispatch_wg(int k, int bn, bool stack, bool narrow, bool halo, const WgMaps& m, float* gw, float* part, const WgParams& p,
                        cudaStream_t st) {
-#define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3, 4>(m, gw, part, p, st)
-#define GIFB200_WGN(KW, BN, HA) launch_wg<KW, BN, false, HA, X3, 2>(m, gw, part, p, st)
+#define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3, 4, RS>(m, gw, part, p, st)
+#define GIFB200_WGN(KW, BN, HA) launch_wg<KW, BN, false, HA, X3, 2, RS>(m, gw, part, p, st)
     if (narrow) {
-        if constexpr (!X3)
-            if (halo) return bn == 64 ? GIFB200_WGN(3, 64, true) : GIFB200_WGN(3, 32, true);
+        if (halo) return bn == 64 ? GIFB200_WGN(3, 64, true) : GIFB200_WGN(3, 32, true);
         if (k == 3) return bn == 64 ? GIFB200_WGN(3, 64, false) : GIFB200_WGN(3, 32, false);
         return bn == 64 ? GIFB200_WGN(1, 64, false) : GIFB200_WGN(1, 32, false);
     }
-    if constexpr (!X3) {
-        if (stack && halo) return bn == 64 ? GIFB200_WG(3, 64, true, true) : GIFB200_WG(3, 32, true, true);
-        if (halo) return bn == 64 ? GIFB200_WG(3, 64, false, true) : GIFB200_WG(3, 32, false, true);
-    }
+    if (stack && halo) return bn == 64 ? GIFB200_WG(3, 64, true, true) : GIFB200_WG(3, 32, true, true);
+    if (halo) return bn == 64 ? GIFB200_WG(3, 64, false, true) : GIFB200_WG(3, 32, false, true);
     if (stack) return bn == 64 ? GIFB200_WG(3, 64, true, false) : GIFB200_WG(3, 32, true, false);
     if (k == 3) return bn == 64 ? GIFB200_WG(3, 64, false, false) : GIFB200_WG(3, 32, false, false);
     return bn == 64 ? GIFB200_WG(1, 64, false, false) : GIFB200_WG(1, 32, false, false);
@@ -507,10 +540,9 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
         if (rc == GIFB200_OK && x3) rc = encode_map(&m.s2, Sb + s_plane, 4, dims, strides, box, swz, dt);
         if (rc != GIFB200_OK) return rc;
     }
-    // GIFB200_WGRAD_HALO: 0 = off, 1 = on (default; fp32 operands only -- the bf16 planes are read by wgmma, which needs
-    // every tap tile to start on a swizzle atom).
+    // GIFB200_WGRAD_HALO: 0 = off, 1 = on (default)
     static const int halo_env = [] { const char* e = getenv("GIFB200_WGRAD_HALO"); return e ? atoi(e) : 1; }();
-    const bool halo = halo_env > 0 && !x3 && mode == 0 && k == 3 && p.pw == kPix;
+    const bool halo = halo_env > 0 && mode == 0 && k == 3 && p.pw == kPix;
     if (!p.s2) {
         const cuuint64_t dims[4] = {static_cast<cuuint64_t>(p.Cb), static_cast<cuuint64_t>(p.Wb), static_cast<cuuint64_t>(p.Hb), static_cast<cuuint64_t>(B)};
         const cuuint64_t strides[3] = {static_cast<cuuint64_t>(p.Cb) * es, static_cast<cuuint64_t>(p.Wb) * p.Cb * es,
@@ -537,8 +569,12 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
         if (rc != GIFB200_OK) return rc;
     }
     if (!x3) { m.s2 = m.s; m.b2 = m.b; }
-    return x3 ? dispatch_wg<true>(k, bn, stack, narrow, halo, m, gw, part, p, st)
-              : dispatch_wg<false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
+    if (!x3) return dispatch_wg<false, false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
+    // GIFB200_WGRAD_X3_RS: 1 = the bf16x3 wgmmas take the S operand from registers (default), 0 = from shared memory like B.
+    // Both issue the same MMAs in the same order into the same accumulators: the results are bitwise the same.
+    static const int rs_env = [] { const char* e = getenv("GIFB200_WGRAD_X3_RS"); return e ? atoi(e) : 1; }();
+    return rs_env > 0 ? dispatch_wg<true, true>(k, bn, stack, narrow, halo, m, gw, part, p, st)
+                      : dispatch_wg<true, false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
 }
 
 }  // namespace gifb200

@@ -126,6 +126,33 @@ GIF_WGMMA_BF16(256, 128, 128, 129, 130, 131, 132, 0)
 GIF_WGMMA_BF16(32, 16, 16, 17, 18, 19, 20, 1)
 GIF_WGMMA_BF16(64, 32, 32, 33, 34, 35, 36, 1)
 
+// bf16, A from registers: a[0..3] = the m64k16 A fragment of thread t of the warpgroup (warp w, lane l, g = l/4, q = l%4):
+// rows 16w + g (a[0], a[2]) and 16w + g + 8 (a[1], a[3]), columns 2q, 2q+1 (a[0], a[1]) and 2q+8, 2q+9 (a[2], a[3]), two
+// bf16 per register, the lower column in the low half (ldmatrix_x4_trans of an MN-major tile gives exactly this).
+// B from a descriptor; Trans<1>: B MN-major.  wgmma reads a[] asynchronously: the registers must not be rewritten before
+// the wgmma_wait that covers the MMA.
+template <int N, int T>
+__device__ __forceinline__ void wgmma_bf16_rs(float* d, const uint32_t* a, uint64_t db, int scale_d, Trans<T>);
+#define GIF_WGMMA_BF16_RS(N, R, A0, A1, A2, A3, S1, S2, T1, TR) \
+    template <> \
+    __device__ __forceinline__ void wgmma_bf16_rs<N>(float* d, const uint32_t* a, uint64_t db, int scale_d, Trans<TR>) { \
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #S2 ", 0;\n" \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" GIF_R##R "}, {%" #A0 ", %" #A1 ", %" #A2 \
+                     ", %" #A3 "}, %" #S1 ", p, 1, 1, %" #T1 ";\n}\n" \
+                     : GIF_F##R \
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TR)); \
+    }
+GIF_WGMMA_BF16_RS(32, 16, 16, 17, 18, 19, 20, 21, 22, 1)
+GIF_WGMMA_BF16_RS(64, 32, 32, 33, 34, 35, 36, 37, 38, 1)
+
+// four 8x8 b16 matrices, transposed: lanes 8i..8i+7 give the row addresses (16 B each) of matrix i, r[i] receives it
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t* r, uint32_t smem_addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(smem_addr)
+                 : "memory");
+}
+
 // warp-level tensor-core MMA, m16n8k8, tf32 operands, fp32 accumulate (the weight-gradient kernel's tf32 mode: its operands
 // are MN-major in shared memory, which wgmma does not accept for 32-bit types, so the fragments are gathered with lds)
 __device__ __forceinline__ void mma_tf32_m16n8k8(float* c, const uint32_t* a, const uint32_t* b) {
