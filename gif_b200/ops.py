@@ -245,10 +245,12 @@ class _Conv(torch.autograd.Function):
     """y = conv(x; W) with W addressed in the physical buffer w[T][R][S] (see gifb200.h)."""
 
     @staticmethod
-    def forward(ctx, x, w, k, mode, flip, transposed, out_hw):
-        x, w = _c(x), _c(w)
+    def forward(ctx, x_arg, w, k, mode, flip, transposed, out_hw):
+        x, w = _c(x_arg), _c(w)
         y, x_used = _conv_raw(x, w, k, mode, flip, transposed, out_hw)
-        ctx.save_for_backward(x_used, w)          # the (possibly tf32-rounded) operand is what wgrad re-reads
+        # the (possibly tf32-rounded) operand is what wgrad re-reads; a rounded copy is outside the autograd graph, so a
+        # recorded (create_graph) backward takes the weight gradient of the input itself (_wgrad_raw rounds it again)
+        ctx.save_for_backward(x_used, w, x_arg if x_used is not x and ctx.needs_input_grad[0] else None)
         ctx.cfg = (k, mode, flip, transposed, tuple(x.shape[1:3]), _is_tf32(x_used))
         c = getattr(x_used, "_gifb200_planes", None)
         ctx.planes = c[1] if c is not None and c[0] == x_used._version else None   # bf16x3: wgrad reuses the split
@@ -257,7 +259,7 @@ class _Conv(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
-        x, w = ctx.saved_tensors
+        x, w, x_arg = ctx.saved_tensors
         k, mode, flip, transposed, in_hw, x_tf32 = ctx.cfg
         _tag(x, x_tf32)
         _carry_planes(x, ctx.planes)
@@ -268,7 +270,8 @@ class _Conv(torch.autograd.Function):
             # adj(S1, f, t) = (S1, !f, !t); adj(S2, f, t) = (T2, f, !t); adj(T2, f, t) = (S2, f, !t)
             gx = _Conv.apply(gy, w, k, _ADJ_MODE[mode], (not flip) if mode == S1 else flip, not transposed, in_hw)
         if ctx.needs_input_grad[1] and _WEIGHT_GRADS[0]:
-            gw = _ConvWgrad.apply(x, gy, k, mode, flip, transposed)
+            xw = x_arg if x_arg is not None and torch.is_grad_enabled() else x
+            gw = _ConvWgrad.apply(xw, gy, k, mode, flip, transposed)
         return gx, gw, None, None, None, None, None
 
 
@@ -301,11 +304,11 @@ class _ConvBiasAct(torch.autograd.Function):
     composed of the differentiable primitives (activation backward from the saved OUTPUT, adjoint conv, wgrad)."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, k, mode, slope, gain, rt, out_hw):
-        x, w = _c(x), _c(w)
+    def forward(ctx, x_arg, w, bias, k, mode, slope, gain, rt, out_hw):
+        x, w = _c(x_arg), _c(w)
         bias_flat = None if bias is None else _c(bias.reshape(-1))
         y, x_used = _conv_raw(x, w, k, mode, False, False, out_hw, (bias_flat, slope, gain, rt))
-        ctx.save_for_backward(x_used, w, y)
+        ctx.save_for_backward(x_used, w, y, x_arg if x_used is not x and ctx.needs_input_grad[0] else None)   # as _Conv
         ctx.cfg = (k, mode, slope, gain, tuple(x.shape[1:3]), _is_tf32(x_used), None if bias is None else bias.shape)
         c = getattr(x_used, "_gifb200_planes", None)
         ctx.planes = c[1] if c is not None and c[0] == x_used._version else None
@@ -314,7 +317,7 @@ class _ConvBiasAct(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
-        x, w, y = ctx.saved_tensors
+        x, w, y, x_arg = ctx.saved_tensors
         k, mode, slope, gain, in_hw, x_tf32, bias_shape = ctx.cfg
         _tag(x, x_tf32)
         _carry_planes(x, ctx.planes)
@@ -350,7 +353,7 @@ class _ConvBiasAct(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             gx = _Conv.apply(gt, w, k, _ADJ_MODE[mode], mode == S1, True, in_hw)
         if ctx.needs_input_grad[1] and _WEIGHT_GRADS[0]:
-            gw = _ConvWgrad.apply(x, gt, k, mode, False, False)
+            gw = _ConvWgrad.apply(x_arg if x_arg is not None and torch.is_grad_enabled() else x, gt, k, mode, False, False)
         return gx, gw, gb, None, None, None, None, None, None
 
 

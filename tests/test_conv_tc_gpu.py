@@ -41,7 +41,7 @@ CASES = [
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 def test_tc_matches_simt(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed):
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + Hs + Ci + mode)
     Hi, Wi = (Hs, Ws) if mode != 1 else (2 * Hs + 1, 2 * Ws + 1)
@@ -123,7 +123,7 @@ def test_splitk_with_fused_epilogue(cuda, B, Hs, Ws, Ci, Co, k, mode, impl):
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", WG_CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 def test_wgrad_tc_matches_simt(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed):
     from gif_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(B * 77 + Hs + Ci + mode)
@@ -170,7 +170,7 @@ def test_split_bf16_planes(cuda):
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 def test_bf16x3_conv_matches_exact_fp32(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed):
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + Hs + Ci + mode + 5)
     Hi, Wi = (Hs, Ws) if mode != 1 else (2 * Hs + 1, 2 * Ws + 1)
@@ -185,7 +185,7 @@ def test_bf16x3_conv_matches_exact_fp32(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, 
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", WG_CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 def test_bf16x3_wgrad_matches_exact_fp32(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed):
     from gif_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(B * 77 + Hs + Ci + mode + 5)

@@ -44,7 +44,7 @@ CASES = [
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 def test_large_tile_tf32_matches_simt(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed):
     from gif_b200 import ops
     x, w = inputs(B, Hs, Ws, Ci, Co, k, mode, transposed, B * 1000 + Hs + Ci + mode, cuda)
@@ -58,7 +58,7 @@ def test_large_tile_tf32_matches_simt(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, tr
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 def test_large_tile_bf16x3_matches_exact_fp32(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed):
     x, w = inputs(B, Hs, Ws, Ci, Co, k, mode, transposed, B * 1000 + Hs + Ci + mode + 5, cuda)
     y_x3 = run(x, w, k, mode, flip, transposed, 3)

@@ -44,7 +44,7 @@ def wgrad(x, gy, k, mode, flip, transposed, impl):
 
 
 @pytest.mark.parametrize("B,Hs,Ws,Ci,Co,k,mode", CASES)
-@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True)])
+@pytest.mark.parametrize("flip,transposed", [(False, False), (True, True), (False, True)])
 @pytest.mark.parametrize("impl", [2, 3])
 def test_narrow_wgrad(cuda, B, Hs, Ws, Ci, Co, k, mode, flip, transposed, impl):
     from gif_b200 import ops
