@@ -34,6 +34,7 @@ SIGNATURES = {
     "gifb200_conv2d_ex": (_i, [_p, _p, _p] + [_i] * 16 + [_p, _i, _p, _sz, _p]),
     "gifb200_pool2d": (_i, [_p, _p] + [_i] * 12 + [_p]),
     "gifb200_resize_bilinear": (_i, [_p, _p, _i, _i, _i, _ll, _ll, _ll, _ll, _i, _i, _i, _f, _f, _i, _p]),
+    "gifb200_resize_bilinear_u8": (_i, [_p, _p, _i, _i, _i, _ll, _i, _i, _i, _f, _f, _i, _p]),
     "gifb200_split_bf16": (_i, [_p, _p, _p, _i, _i, _i, _p]),
     "gifb200_upfirdn2d": (_i, [_p, _p, _p] + [_i] * 14 + [_p]),
     "gifb200_bias_act": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _f, _f, _i, _p]),

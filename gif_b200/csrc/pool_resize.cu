@@ -1,4 +1,5 @@
-// gifb200_pool2d and gifb200_resize_bilinear: the pooling layers and the input resize of the FID InceptionV3.
+// gifb200_pool2d, gifb200_resize_bilinear and gifb200_resize_bilinear_u8: the pooling layers and the input resize of the FID
+// InceptionV3.
 #include "common.cuh"
 
 namespace gifb200 {
@@ -44,8 +45,24 @@ __device__ __forceinline__ void src_index(int d, double scale, int in, int& i0, 
     l1 = static_cast<float>(s - i0);
 }
 
-// x (B,3,H,W) through element strides -> y (B,Ho,Wo,Cy) channels-last, channels 3..Cy-1 zero; v -> a*v + b
-__global__ void __launch_bounds__(256) resize_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
+// v / 255 in float32 for every byte, rounded to nearest as numpy's float32 `/= 255` (IEEE division), evaluated at compile
+// time: a division in the kernel brings its slow-path call, and with it a stack frame and spills.
+struct U8Unit {
+    float v[256];
+    constexpr U8Unit() : v() {
+        for (int i = 0; i < 256; ++i) v[i] = static_cast<float>(i) / 255.f;
+    }
+};
+__device__ constexpr U8Unit kU8Unit{};
+
+// a source sample as the float kernel sees it: fp32 as stored; uint8 as v / 255
+__device__ __forceinline__ float load_src(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float load_src(const uint8_t* p) { return __ldg(kU8Unit.v + __ldg(p)); }
+
+// x (B,3,H,W) through element strides -> y (B,Ho,Wo,Cy) channels-last, channels 3..Cy-1 zero; v -> a*v + b.  Both source
+// types run the same arithmetic after load_src, so the uint8 result is bitwise the float kernel's on x / 255.
+template <typename T>
+__global__ void __launch_bounds__(256) resize_kernel(const T* __restrict__ x, float* __restrict__ y, int B, int H, int W,
                                                      long long sb, long long sc, long long sh, long long sw, int Ho, int Wo,
                                                      int Cy, float a, float bb, int rtf32) {
     const long long n = static_cast<long long>(B) * Ho * Wo;
@@ -59,9 +76,9 @@ __global__ void __launch_bounds__(256) resize_kernel(const float* __restrict__ x
         src_index(xo, sx, W, x0, x1, lx);
         float* dst = y + e * Cy;
         for (int c = 0; c < 3; ++c) {
-            const float* p = x + b * sb + c * sc;
-            const float v00 = __ldg(p + y0 * sh + x0 * sw), v01 = __ldg(p + y0 * sh + x1 * sw);
-            const float v10 = __ldg(p + y1 * sh + x0 * sw), v11 = __ldg(p + y1 * sh + x1 * sw);
+            const T* p = x + b * sb + c * sc;
+            const float v00 = load_src(p + y0 * sh + x0 * sw), v01 = load_src(p + y0 * sh + x1 * sw);
+            const float v10 = load_src(p + y1 * sh + x0 * sw), v11 = load_src(p + y1 * sh + x1 * sw);
             const float v = (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
             const float o = a * v + bb;
             dst[c] = rtf32 ? round_tf32(o) : o;
@@ -99,8 +116,21 @@ extern "C" int gifb200_resize_bilinear(const float* x, float* y, int B, int H, i
     const long long n = static_cast<long long>(B) * Ho * Wo;
     int blocks = cdiv(n, 256);
     if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
-    resize_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, y, B, H, W, stride_b, stride_c, stride_h, stride_w, Ho,
-                                                                        Wo, Cy, scale, shift, round_tf32);
+    resize_kernel<float><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, y, B, H, W, stride_b, stride_c, stride_h,
+                                                                               stride_w, Ho, Wo, Cy, scale, shift, round_tf32);
     GIFB200_LAUNCH_CHECK("resize_kernel");
+    return GIFB200_OK;
+}
+
+extern "C" int gifb200_resize_bilinear_u8(const uint8_t* x, float* y, int B, int H, int W, long long stride_b, int Ho, int Wo,
+                                          int Cy, float scale, float shift, int round_tf32, gifb200_stream_t stream) {
+    GIFB200_REQUIRE(B > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Cy >= 3, GIFB200_E_SHAPE,
+                    "resize_bilinear_u8: positive sizes and Cy >= 3");
+    const long long n = static_cast<long long>(B) * Ho * Wo;
+    int blocks = cdiv(n, 256);
+    if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+    resize_kernel<uint8_t><<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, y, B, H, W, stride_b, 1, 3ll * W, 3, Ho, Wo,
+                                                                                 Cy, scale, shift, round_tf32);
+    GIFB200_LAUNCH_CHECK("resize_kernel<u8>");
     return GIFB200_OK;
 }

@@ -79,7 +79,7 @@ def compute_activation_batch(model, batch):
 class FidComputer:
     """compute_fid.py:10-87.  ``model``: the FID Inception network, or None with ``inception_weights`` to build the native one
     for ``dims`` (see the module docstring); ``true_img_stats_dir`` holds the reference's ``ffhq_{R}X{R}_fid_stats.npz`` files
-    (mu, sigma)."""
+    (mu, sigma), computed from the PNGs in ``database_root_dir`` when missing (``compute_true_img_response``)."""
 
     def __init__(self, database_root_dir=None, true_img_stats_dir=None, model=None, dims=2048, device=None,
                  inception_weights=None):
@@ -99,13 +99,23 @@ class FidComputer:
         self.current_resolution = None
 
     def compute_true_img_response(self, resolution):
-        """compute_fid.py:26-46: the pre-computed statistics of the real images at this resolution."""
+        """compute_fid.py:26-46: the statistics of the real images at this resolution.  Loaded from
+        ``true_img_stats_dir/ffhq_{R}X{R}_fid_stats.npz`` when it exists; otherwise computed from ``database_root_dir/*.png``
+        with this computer's network (``fid_real.real_image_statistics``: sorted file names, the reference's selection and
+        resize rules) and, when ``true_img_stats_dir`` is set, written there atomically for the next run."""
         path = os.path.join(self.true_img_stats_dir or "", f"ffhq_{resolution}X{resolution}_fid_stats.npz")
-        if not os.path.exists(path):
-            raise FileNotFoundError(f"{path}: statistics of the real images not found (the reference computes them from "
-                                    f"{self.true_data_loc}/*.png with the same network and caches them there)")
-        with np.load(path) as f:
-            self.m_t, self.s_t = f["mu"][:], f["sigma"][:]
+        if os.path.exists(path):
+            with np.load(path) as f:
+                self.m_t, self.s_t = f["mu"][:], f["sigma"][:]
+            return
+        if self.true_data_loc is None:
+            raise FileNotFoundError(f"{path}: statistics of the real images not found, and no image folder "
+                                    "(database_root_dir) to compute them from")
+        from .fid_real import real_image_statistics, save_statistics
+        mu, sigma = real_image_statistics(self.true_data_loc, resolution, self.model, self.dims, device=self.device)
+        self.m_t, self.s_t = mu.cpu().numpy(), sigma.cpu().numpy()
+        if self.true_img_stats_dir is not None:
+            save_statistics(path, self.m_t, self.s_t)
 
     def compute_sats_given_img_tensor(self, imag_tensor, batch_size=32):
         """compute_fid.py:48-82: float32 images are range-normalised to [0,1] over the WHOLE tensor, uint8 divided by 255."""

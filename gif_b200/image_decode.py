@@ -449,19 +449,26 @@ def bicubic_coeffs(in_size, out_size):
     return out
 
 
+@lru_cache(maxsize=64)
+def _bicubic_coeffs_device(W, H, size, device):
+    """``bicubic_coeffs`` of both passes on the device, uploaded once per shape: a per-call upload would wait for the
+    stream (a blocking host-to-device copy) and stall a pipeline that keeps the device busy."""
+    ch, cv = bicubic_coeffs(W, size), bicubic_coeffs(H, size)
+    return torch.from_numpy(np.concatenate([ch.ravel(), cv.ravel()])).to(device), ch.size, ch.shape[1] - 2, cv.shape[1] - 2
+
+
 def resize_bicubic_u8(x, size, tmp=None, out=None):
     """uint8 (B, H, W, 3) or (H, W, 3) CUDA tensor -> (B, size, size, 3): Pillow's ``Image.resize((size, size))`` (bicubic),
     bit for bit."""
     squeeze = x.dim() == 3
     xb = x.unsqueeze(0) if squeeze else x
     B, H, W, _ = xb.shape
-    ch, cv = bicubic_coeffs(W, size), bicubic_coeffs(H, size)
-    coef = torch.from_numpy(np.concatenate([ch.ravel(), cv.ravel()])).to(x.device)
+    coef, n_h, ks_h, ks_v = _bicubic_coeffs_device(W, H, size, x.device)
     tmp = torch.empty(B, H, size, 3, dtype=torch.uint8, device=x.device) if tmp is None else tmp
     out = torch.empty(B, size, size, 3, dtype=torch.uint8, device=x.device) if out is None else out
     _lib.check(_lib.lib.gifb200_resize_bicubic_u8(xb.contiguous().data_ptr(), tmp.data_ptr(), out.data_ptr(), coef.data_ptr(),
-                                                  coef.data_ptr() + 4 * ch.size, B, H, W, size, size, ch.shape[1] - 2,
-                                                  cv.shape[1] - 2, _lib.stream()), "resize_bicubic_u8")
+                                                  coef.data_ptr() + 4 * n_h, B, H, W, size, size, ks_h, ks_v, _lib.stream()),
+               "resize_bicubic_u8")
     return out[0] if squeeze else out
 
 

@@ -163,8 +163,9 @@ class _FoldedConv(nn.Module):
 
 
 class InceptionV3(nn.Module):
-    """pytorch_fid.InceptionV3 (inception.py:17-164) on gif_b200 kernels, forward only: (B,3,H,W) in [0,1] -> list of the
-    requested blocks' feature maps, NCHW views of channels-last storage, sorted by block index."""
+    """pytorch_fid.InceptionV3 (inception.py:17-164) on gif_b200 kernels, forward only: (B,3,H,W) in [0,1] (or uint8
+    (B,H,W,3), see ``forward``) -> list of the requested blocks' feature maps, NCHW views of channels-last storage, sorted
+    by block index."""
 
     DEFAULT_BLOCK_INDEX = 3
     BLOCK_INDEX_BY_DIM = {64: 0, 192: 1, 768: 2, 2048: 3}
@@ -279,11 +280,15 @@ class InceptionV3(nn.Module):
         return s.view(B, 1, 1, C)
 
     def forward(self, inp):
+        """``inp``: (B,3,H,W) float32 in [0,1], or uint8 RGB (B,H,W,3) on the device, read as v / 255 by the input resize
+        (``ops.resize_bilinear_u8``: fid_score.py:106-112's float batch without materialising it)."""
         if torch.is_grad_enabled() and inp.requires_grad:
             raise RuntimeError("gif_b200's InceptionV3 is forward-only: the input must not require grad")
-        H, W = (299, 299) if self.resize_input else tuple(inp.shape[2:])
+        u8 = inp.dtype == torch.uint8
+        H, W = (299, 299) if self.resize_input else tuple(inp.shape[1:3] if u8 else inp.shape[2:])
         scale, shift = (2.0, -1.0) if self.normalize_input else (1.0, 0.0)
-        x = ops.resize_bilinear(inp, (H, W), 32, scale, shift, round_tf32=ops.tf32_enabled())
+        resize = ops.resize_bilinear_u8 if u8 else ops.resize_bilinear
+        x = resize(inp, (H, W), 32, scale, shift, round_tf32=ops.tf32_enabled())
         outp = []
         for i in range(self.last_needed_block + 1):
             x = self._block(i, x)

@@ -15,7 +15,7 @@ import weakref
 
 import torch
 
-from ._lib import check, lib, ptr, require_cuda, stream
+from ._lib import GifB200Error, check, lib, ptr, require_cuda, stream
 
 S1, S2, T2 = 0, 1, 2          # conv modes of gifb200_conv2d
 _ADJ_MODE = {S1: S1, S2: T2, T2: S2}
@@ -1140,6 +1140,23 @@ def resize_bilinear(x, size, channels=32, scale=1.0, shift=0.0, round_tf32=False
     sb, sc, sh, sw = x.stride()
     check(lib.gifb200_resize_bilinear(ptr(x), ptr(y), B, H, W, sb, sc, sh, sw, size[0], size[1], channels, float(scale),
                                       float(shift), int(round_tf32), stream()), "gifb200_resize_bilinear")
+    return y
+
+
+def resize_bilinear_u8(x, size, channels=32, scale=1.0, shift=0.0, round_tf32=False):
+    """``resize_bilinear`` of uint8 RGB images x (B,H,W,3) read as v / 255 (IEEE division) -- bitwise equal to
+    ``resize_bilinear(x.permute(0,3,1,2).float() / 255)`` with a true division -- without writing that float batch
+    (gifb200_resize_bilinear_u8).  Rows must be dense; the batch stride is free."""
+    if not x.is_cuda:
+        raise GifB200Error(f"resize_bilinear_u8 runs on CUDA tensors only; got a {x.device} tensor")
+    if x.dtype != torch.uint8 or x.dim() != 4 or x.shape[3] != 3:
+        raise ValueError(f"resize_bilinear_u8 takes uint8 (B,H,W,3) images, got {x.dtype} {tuple(x.shape)}")
+    B, H, W, _ = x.shape
+    if x.stride()[1:] != (3 * W, 3, 1):
+        raise ValueError(f"resize_bilinear_u8: rows must be dense (strides (*, {3 * W}, 3, 1)), got {x.stride()}")
+    y = torch.empty((B, size[0], size[1], channels), dtype=torch.float32, device=x.device)
+    check(lib.gifb200_resize_bilinear_u8(ptr(x), ptr(y), B, H, W, x.stride(0), size[0], size[1], channels, float(scale),
+                                         float(shift), int(round_tf32), stream()), "gifb200_resize_bilinear_u8")
     return y
 
 

@@ -57,6 +57,16 @@ def flat(h, w, seed):
     return Image.fromarray(a)
 
 
+def png_folder(root, n, size, seed=0):
+    """``n`` photo-like RGB PNGs of size x size written by Pillow as ``root/{i:05d}.png`` (FFHQ's naming); returns the paths."""
+    os.makedirs(root, exist_ok=True)
+    paths = []
+    for i in range(n):
+        paths.append(os.path.join(str(root), f"{i:05d}.png"))
+        photo(size, size, seed + i).save(paths[-1], "PNG")
+    return paths
+
+
 def build_lmdbs(root, n, R, rr):
     """Real and render LMDBs as the reference's writers build them: LANCZOS resize + centre crop + JPEG q100, PNG renders."""
     from gif_b200.data import image_key, normal_map_key, write_lmdb

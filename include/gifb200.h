@@ -130,6 +130,12 @@ int gifb200_pool2d(const float* x, float* y, int B, int Hi, int Wi, int C, int H
 int gifb200_resize_bilinear(const float* x, float* y, int B, int H, int W, long long stride_b, long long stride_c,
                             long long stride_h, long long stride_w, int Ho, int Wo, int Cy, float scale, float shift,
                             int round_tf32, gifb200_stream_t stream);
+/* The same resize of uint8 RGB images x (B,H,W,3) channels-last, rows dense, image b at x + b*stride_b (the layout of
+ * gifb200_png_unfilter's and gifb200_resize_bicubic_u8's output): each sample is read as v / 255 (float32, IEEE division, as
+ * numpy's `images /= 255` in my_utils/pytorch_fid/fid_score.py:112), then the arithmetic of gifb200_resize_bilinear, so y is
+ * bitwise gifb200_resize_bilinear of that float batch, which is never written. */
+int gifb200_resize_bilinear_u8(const uint8_t* x, float* y, int B, int H, int W, long long stride_b, int Ho, int Wo, int Cy,
+                               float scale, float shift, int round_tf32, gifb200_stream_t stream);
 
 /* Two-term bf16 expansion of an fp32 tensor (B, P pixels, C channels, channels-last), optionally fused with the style
  * modulation of ModulatedConv2d (cl.py:311-313 in the modulate-input form): v = x[b,p,c] * (s ? s[b,c] : 1);
