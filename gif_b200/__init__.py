@@ -12,7 +12,7 @@ import importlib
 import sys
 
 _LAZY = ("_lib", "ops", "losses", "rasterize", "distributed", "checkpoint", "train_step", "render", "flame", "texture_space",
-         "inference", "model")
+         "inference", "model", "eye_centering", "sampler")
 
 
 def __getattr__(name):

@@ -64,6 +64,7 @@ SIGNATURES = {
     "gifb200_rasterize_bwd": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "gifb200_flame_lbs_workspace_bytes": (_sz, [_i, _i]),
     "gifb200_flame_lbs": (_i, [_p] * 11 + [_i] * 4 + [_p, _sz, _p]),
+    "gifb200_eye_camera": (_i, [_p, _p] + [_i] * 4 + [_f] * 4 + [_p]),
     "gifb200_flametex": (_i, [_p] * 4 + [_i] * 4 + [_p]),
     "gifb200_texture_steal_fwd": (_i, [_p] * 9 + [_i] * 6 + [_p]),
     "gifb200_texture_steal_bwd": (_i, [_p] * 7 + [_i] * 6 + [_p]),
@@ -72,6 +73,7 @@ SIGNATURES = {
     "gifb200_png_unfilter": (_i, [_p, _p, _i, _i, _p, _p, _p]),
     "gifb200_resize_bicubic_u8": (_i, [_p] * 5 + [_i] * 7 + [_p]),
     "gifb200_u8_to_unit": (_i, [_p, _p, _i, _i, _i, _ll, _p]),
+    "gifb200_image_to_u8": (_i, [_p, _p, _i, _i, _i, _ll, _ll, _ll, _ll, _p]),
 }
 
 

@@ -49,13 +49,18 @@ class DecaConditionRenderer:
         """deca (B, >=236) float32 CUDA, RAW parameter rows (not normalised labels) -> uint8 (2B, S, S, 3): planes 0..B-1
         the textured renders, planes B..2B-1 the normal maps.  ``out``: an optional tensor of that shape to write into."""
         p = split_deca(deca.float())
-        B, S = deca.shape[0], self.image_size
         verts, _ = self.flame.decode_vertices(p["shape"].contiguous(), p["exp"].contiguous(), p["pose"].contiguous())
-        albedo = self.flametex(p["tex"])
-        trans = batch_orth_proj(verts, p["cam"].contiguous())                       # gif_helper.py:25-27
+        return self.render_vertices_u8(verts, p["cam"].contiguous(), self.flametex(p["tex"]), p["lit"], out)
+
+    @torch.no_grad()
+    def render_vertices_u8(self, verts, cam, albedo, lights, out=None):
+        """The render of ``render_u8`` from decoded vertices (B,V,3), cameras (B,3), albedo (B,3,T,T) and lights (B,9,3):
+        -> uint8 (2B, S, S, 3), textured renders then normal maps (into ``out`` when given)."""
+        B, S = verts.shape[0], self.image_size
+        trans = batch_orth_proj(verts, cam)                                          # gif_helper.py:25-27
         trans[:, :, 1:] = -trans[:, :, 1:]
-        out = torch.empty(2 * B, S, S, 3, dtype=torch.uint8, device=deca.device) if out is None else out
-        self.renderer(verts, trans, albedo, p["lit"], want_cond=False, cond_u8=out)
+        out = torch.empty(2 * B, S, S, 3, dtype=torch.uint8, device=verts.device) if out is None else out
+        self.renderer(verts, trans, albedo, lights, want_cond=False, cond_u8=out)
         return out
 
     def __call__(self, deca):

@@ -197,6 +197,38 @@ extern "C" int gifb200_flame_lbs(const float* betas, const float* pose, const fl
     return GIFB200_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- eye-centred camera
+// position_to_given_location (my_utils/eye_centering.py:35-66): the weak-perspective camera (s, bx, by) that puts the two
+// eye vertices at fixed image positions.  The reference solves  d = (s, s bx, s by) M  with  M = [[e1x e2x e1y e2y],
+// [1 1 0 0], [0 0 1 1]]  by a float32 pseudo-inverse per row; for a full-rank M that least-squares solution is
+//     s = (dex dx + dey dy) / (dex^2 + dey^2),  s bx = (x1 + x2)/2 - s (e1x + e2x)/2,  s by likewise,
+// with dex = e1x - e2x, dx = x1 - x2 (y likewise), evaluated here in float64 and rounded once.  cam = (-s, bx, by).
+// A row whose eyes coincide in x and y has no unique camera: 0/0 makes it NaN (the reference divides by zero there too).
+__global__ void __launch_bounds__(128) eye_camera_kernel(const float* __restrict__ verts, float* __restrict__ cam, int B, int V,
+                                                         int i1, int i2, double x1, double x2, double y1, double y2) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const float* v = verts + static_cast<long long>(b) * V * 3;
+    const double e1x = v[i1 * 3 + 0], e1y = v[i1 * 3 + 1], e2x = v[i2 * 3 + 0], e2y = v[i2 * 3 + 1];
+    const double dex = e1x - e2x, dey = e1y - e2y;
+    const double s = (dex * (x1 - x2) + dey * (y1 - y2)) / (dex * dex + dey * dey);
+    const double sbx = 0.5 * (x1 + x2) - s * (0.5 * (e1x + e2x));
+    const double sby = 0.5 * (y1 + y2) - s * (0.5 * (e1y + e2y));
+    cam[b * 3 + 0] = static_cast<float>(-s);
+    cam[b * 3 + 1] = static_cast<float>(sbx / s);
+    cam[b * 3 + 2] = static_cast<float>(sby / s);
+}
+
+extern "C" int gifb200_eye_camera(const float* verts, float* cam, int B, int V, int i1, int i2, float x1, float x2, float y1,
+                                  float y2, gifb200_stream_t stream) {
+    GIFB200_REQUIRE(B >= 0 && V > 0, GIFB200_E_SHAPE, "eye_camera: bad shape");
+    GIFB200_REQUIRE(i1 >= 0 && i1 < V && i2 >= 0 && i2 < V, GIFB200_E_SHAPE, "eye_camera: eye vertex index outside 0..V-1");
+    if (B == 0) return GIFB200_OK;
+    eye_camera_kernel<<<cdiv(B, 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(verts, cam, B, V, i1, i2, x1, x2, y1, y2);
+    GIFB200_LAUNCH_CHECK("eye_camera_kernel");
+    return GIFB200_OK;
+}
+
 // ------------------------------------------------------------------------------------------------------------ FLAMETex
 // FLAMETex.forward (models/FLAME.py:237-242): mean + basis . texcode, reshaped to side x side x 3, F.interpolate to T x T in
 // the default nearest mode (source index min(floor(dst * side / T), side - 1)), RGB -> BGR -- evaluated only at the texels

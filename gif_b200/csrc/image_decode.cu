@@ -351,6 +351,25 @@ __global__ void __launch_bounds__(256) u8_to_unit_kernel(const uint8_t* x, float
     }
 }
 
+// The inverse direction, as the reference saves generated images (my_utils/generic_utils.py:134-164 after the
+// clamp to [-1, 1] of the sampling scripts): uint8(clip(fl(fl(a + 1) * 0.5), 0, 1) * 255) in float32, truncated, with
+// a = clamp(x, -1, 1).  The explicit round-to-nearest intrinsics keep nvcc from contracting the steps into an FMA.
+// x is any strided (B, 3, H, W) float32 view; y is dense (B, H, W, 3).  NaN inputs are outside the contract.
+__global__ void __launch_bounds__(256) image_to_u8_kernel(const float* x, uint8_t* y, int B, int H, int W, long long sb,
+                                                          long long sc, long long sh, long long sw) {
+    const long long HW = static_cast<long long>(H) * W, n = B * HW;
+    for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < n;
+         e += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long b = e / HW, p = e - b * HW, h = p / W, w = p - h * W;
+        const float* src = x + b * sb + h * sh + w * sw;
+        for (int c = 0; c < 3; ++c) {
+            const float a = fminf(fmaxf(src[c * sc], -1.f), 1.f);
+            const float t = fminf(fmaxf(__fmul_rn(__fadd_rn(a, 1.f), 0.5f), 0.f), 1.f);
+            y[e * 3 + c] = static_cast<uint8_t>(static_cast<int>(__fmul_rn(t, 255.f)));
+        }
+    }
+}
+
 int grid_for(long long n) {
     int blocks = cdiv(n, 256);
     return blocks > kNumSMs * 16 ? kNumSMs * 16 : (blocks < 1 ? 1 : blocks);
@@ -444,5 +463,14 @@ extern "C" int gifb200_u8_to_unit(const uint8_t* x, float* y, int B, int H, int 
     u8_to_unit_kernel<<<grid_for(static_cast<long long>(B) * H * W), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, y, B, H * W,
                                                                                                                  y_batch_stride);
     GIFB200_LAUNCH_CHECK("u8_to_unit_kernel");
+    return GIFB200_OK;
+}
+
+extern "C" int gifb200_image_to_u8(const float* x, uint8_t* y, int B, int H, int W, long long stride_b, long long stride_c,
+                                   long long stride_h, long long stride_w, gifb200_stream_t stream) {
+    GIFB200_REQUIRE(B > 0 && H > 0 && W > 0, GIFB200_E_SHAPE, "image_to_u8: positive sizes");
+    image_to_u8_kernel<<<grid_for(static_cast<long long>(B) * H * W), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        x, y, B, H, W, stride_b, stride_c, stride_h, stride_w);
+    GIFB200_LAUNCH_CHECK("image_to_u8_kernel");
     return GIFB200_OK;
 }

@@ -480,3 +480,18 @@ def u8_to_unit(x, out):
         raise ValueError("u8_to_unit: out must be a float32 (B, 3, H, W) view with dense channel planes")
     _lib.check(_lib.lib.gifb200_u8_to_unit(x.data_ptr(), out.data_ptr(), B, H, W, out.stride(0), _lib.stream()), "u8_to_unit")
     return out
+
+
+def image_to_u8(x, out=None):
+    """float32 (B, 3, H, W) CUDA view with any strides (the generator's NCHW view of channels-last storage included) ->
+    uint8 (B, H, W, 3): the bytes the reference's sampling scripts save, ``uint8(clip((clamp(x, -1, 1) + 1) / 2, 0, 1) * 255)``
+    in float32 (the inverse direction of ``u8_to_unit``).  NaN inputs are outside the contract."""
+    if x.dim() != 4 or x.shape[1] != 3 or x.dtype != torch.float32 or not x.is_cuda:
+        raise ValueError(f"image_to_u8: x must be a float32 CUDA (B, 3, H, W) tensor, got {x.dtype} {tuple(x.shape)} on {x.device}")
+    B, _, H, W = x.shape
+    if out is None:
+        out = torch.empty(B, H, W, 3, dtype=torch.uint8, device=x.device)
+    elif out.shape != (B, H, W, 3) or out.dtype != torch.uint8 or not out.is_contiguous():
+        raise ValueError(f"image_to_u8: out must be a contiguous uint8 ({B}, {H}, {W}, 3) tensor")
+    _lib.check(_lib.lib.gifb200_image_to_u8(x.data_ptr(), out.data_ptr(), B, H, W, *x.stride(), _lib.stream()), "image_to_u8")
+    return out

@@ -320,6 +320,14 @@ int gifb200_flame_lbs(const float* betas, const float* pose, const float* v_temp
                       const float* lbs_weights, float* verts, float* joints, int B, int V, int NB, int NJ, void* ws,
                       size_t ws_bytes, gifb200_stream_t stream);
 
+/* Eye-centred camera, position_to_given_location (my_utils/eye_centering.py:35-66): for each row of verts (B,V,3), the
+ * weak-perspective camera cam (B,3) = (-s, bx, by) that maps the eye vertices i1, i2 to the image positions (x1, y1),
+ * (x2, y2) in the least-squares sense of the reference's pseudo-inverse: s = (dex dx + dey dy) / (dex^2 + dey^2),
+ * s bx = (x1 + x2)/2 - s (e1x + e2x)/2 (y likewise), dex = e1x - e2x, dx = x1 - x2; float64, rounded once to float32.
+ * A row whose two eye vertices coincide in x and y has no unique camera and gets NaN.  0 <= i1, i2 < V. */
+int gifb200_eye_camera(const float* verts, float* cam, int B, int V, int i1, int i2, float x1, float x2, float y1, float y2,
+                       gifb200_stream_t stream);
+
 /* FLAMETex.forward (models/FLAME.py:237-242) at the texels its nearest resize keeps: albedo (B,3,T,T) BGR,
  * albedo[b,2-c,y,x] = mean[k] + sum_j basis[k,j] texcode[b,j] with k = (sy*side + sx)*3 + c, sy = min(floor(y*side/T),
  * side-1) (likewise sx) in float32 as F.interpolate's nearest mode computes it.  texcode (B,n), mean (side*side*3),
@@ -379,6 +387,13 @@ int gifb200_resize_bicubic_u8(const uint8_t* x, uint8_t* tmp, uint8_t* y, const 
 /* uint8 RGB (B, H, W, 3) -> y[b*y_batch_stride + c*H*W + p] = (v / 255 - 0.5) / 0.5 (float32, IEEE division): three
  * channels of an NCHW batch, so a render and a normal map go straight into their slices of the condition tensor. */
 int gifb200_u8_to_unit(const uint8_t* x, float* y, int B, int H, int W, long long y_batch_stride, gifb200_stream_t stream);
+
+/* Image bytes as the reference's sampling scripts save them (generic_utils.save_set_of_images after clamp to [-1, 1]):
+ * y[b,h,w,c] = uint8(clip(fl(fl(a + 1) * 0.5), 0, 1) * 255), a = clamp(x[b,c,h,w], -1, 1), in float32 with each step
+ * rounded (no FMA), truncated to uint8.  x: any (B, 3, H, W) float32 view, strides in elements (so the generator's NCHW
+ * view of channels-last storage is read in place); y: dense uint8 (B, H, W, 3).  NaN inputs are outside the contract. */
+int gifb200_image_to_u8(const float* x, uint8_t* y, int B, int H, int W, long long stride_b, long long stride_c,
+                        long long stride_h, long long stride_w, gifb200_stream_t stream);
 
 #ifdef __cplusplus
 }
