@@ -5,9 +5,9 @@
 //   K = 32 input channels per pipeline stage (one 128-byte swizzle row of fp32), taps x Ci/32 stages per tile.
 //   * A operand: the activation tensor itself (channels-last fp32) -- no im2col buffer.  Each tap is the same TMA box
 //     shifted by the tap offset; TMA's out-of-bounds zero fill implements the padding.  Stride-2 convolutions (S2)
-//     read through a 5-D view that splits W into (parity, W/2) and load one site row per TMA issue; transposed
-//     stride-2 convolutions (T2) run as 4 output phases (Y%2, X%2), each an ordinary stride-1 gather with its own
-//     subset of the 9 taps, and write with output stride 2.
+//     read through a 5-D view that splits W into (parity, W/2), one box with traversal stride 2 along the input rows;
+//     transposed stride-2 convolutions (T2) run as 4 output phases (Y%2, X%2), each an ordinary stride-1 gather with its
+//     own subset of the 9 taps, and write with output stride 2.
 //   * B operand: the tap-major weights [T][Co][Ci] staged once per call into the workspace (honouring flip /
 //     transposed, rounded to tf32), K-major, 128B swizzle.
 //   * Both operands are K-major SWIZZLE_128B; each of two consumer warpgroups issues one wgmma.m64nNk8.tf32 per m64 row
@@ -43,7 +43,7 @@ struct TcParams {
     int wt, ht, nt;         // tile box (wt*ht*nt == BM)
     int tiles_x, tiles_y;   // tiles per image group
     int Ci, Co;
-    int s2;                 // 1: A loads go through the 5-D parity view, one site row per TMA issue
+    int s2;                 // 0: the A tile is one 4-D box; 1: one 5-D box of the parity view (stride-2 convolutions)
     int Ho, Wo;             // output tensor spatial size
     int oys, oxs;           // output pixel = site * o?s + o?0
     int nphase;
@@ -136,10 +136,8 @@ __global__ void __launch_bounds__(TileCfg<BM, BN>::kThreads, TileCfg<BM, BN>::kM
 
     if (warp >= kConsumerWarps) {
         if constexpr (L::kLarge) setmaxnreg_dec<kProducerRegs>();
-        if (warp != kConsumerWarps) return;
-        // ===================== TMA producer =====================
-        // Lane 0 owns the barriers.  In stride-2 row mode the A tile is nt*ht separate row boxes (the parity view cannot be
-        // one box): the 32 lanes issue them in parallel.
+        if (warp != kConsumerWarps || lane != 0) return;
+        // ===================== TMA producer (one thread) =====================
         int stage = 0;
         uint32_t ph = 0;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -156,42 +154,20 @@ __global__ void __launch_bounds__(TileCfg<BM, BN>::kThreads, TileCfg<BM, BN>::kM
                 const int tap = it / kchunks, c0 = (it % kchunks) * kBlockK;
                 uint8_t* a_dst = smem + stage * L::kStageBytes;
                 uint8_t* b_dst = a_dst + kATileBytes;
-                if (lane == 0) {
-                    mbar_wait(&empty_bar[stage], ph ^ 1);
-                    mbar_expect_tx(&full_bar[stage], L::kStageBytes);
-                }
-                __syncwarp();
+                mbar_wait(&empty_bar[stage], ph ^ 1);
+                mbar_expect_tx(&full_bar[stage], L::kStageBytes);
                 const int dy = p.tap_dy[phase][tap], dx = p.tap_dx[phase][tap];
                 // X3: the hi plane's tile fills the first half of the A (B) slot, the lo plane's tile the second half
                 if (!p.s2) {
-                    if (lane == 0) {
-                        tma_load_4d(a_dst, &map_a, &full_bar[stage], c0, x0 + dx, y0 + dy, n0);
-                        if (X3) tma_load_4d(a_dst + kATileBytes / 2, &map_a2, &full_bar[stage], c0, x0 + dx, y0 + dy, n0);
-                    }
-                } else if (p.s2 == 2) {
-                    // the nt x ht rows of the tile through ONE 5-D box per plane: traversal stride 2 along the input rows
-                    if (lane == 0) {
-                        const int par = p.tap_par[phase][tap];
-                        tma_load_5d(a_dst, &map_a, &full_bar[stage], c0, par, x0 + dx, y0 * p.in_sy + dy, n0);
-                        if (X3) tma_load_5d(a_dst + kATileBytes / 2, &map_a2, &full_bar[stage], c0, par, x0 + dx, y0 * p.in_sy + dy, n0);
-                    }
+                    tma_load_4d(a_dst, &map_a, &full_bar[stage], c0, x0 + dx, y0 + dy, n0);
+                    if (X3) tma_load_4d(a_dst + kATileBytes / 2, &map_a2, &full_bar[stage], c0, x0 + dx, y0 + dy, n0);
                 } else {
                     const int par = p.tap_par[phase][tap];
-                    const int row_bytes = p.wt * kBlockK * (X3 ? 2 : 4);
-                    const int rows = p.nt * p.ht;
-                    for (int r = lane; r < rows; r += 32) {
-                        const int n = r / p.ht, h = r - n * p.ht;
-                        tma_load_5d(a_dst + r * row_bytes, &map_a, &full_bar[stage], c0, par, x0 + dx,
-                                    (y0 + h) * p.in_sy + dy, n0 + n);
-                        if (X3)
-                            tma_load_5d(a_dst + kATileBytes / 2 + r * row_bytes, &map_a2, &full_bar[stage], c0, par, x0 + dx,
-                                        (y0 + h) * p.in_sy + dy, n0 + n);
-                    }
+                    tma_load_5d(a_dst, &map_a, &full_bar[stage], c0, par, x0 + dx, y0 * p.in_sy + dy, n0);
+                    if (X3) tma_load_5d(a_dst + kATileBytes / 2, &map_a2, &full_bar[stage], c0, par, x0 + dx, y0 * p.in_sy + dy, n0);
                 }
-                if (lane == 0) {
-                    tma_load_3d(b_dst, &map_b, &full_bar[stage], c0, nblk * BN, p.tap_w[phase][tap]);
-                    if (X3) tma_load_3d(b_dst + L::kBTileBytes / 2, &map_b2, &full_bar[stage], c0, nblk * BN, p.tap_w[phase][tap]);
-                }
+                tma_load_3d(b_dst, &map_b, &full_bar[stage], c0, nblk * BN, p.tap_w[phase][tap]);
+                if (X3) tma_load_3d(b_dst + L::kBTileBytes / 2, &map_b2, &full_bar[stage], c0, nblk * BN, p.tap_w[phase][tap]);
                 if (++stage == kStages) { stage = 0; ph ^= 1; }
             }
         }
@@ -574,13 +550,11 @@ int conv2d_tc(const float* x, const float* w, float* y, int B, int Hi, int Wi, i
         const cuuint64_t strides[4] = {static_cast<cuuint64_t>(Ci) * es, static_cast<cuuint64_t>(Ci) * 2 * es,
                                        static_cast<cuuint64_t>(Wi) * Ci * es, static_cast<cuuint64_t>(Hi) * Wi * Ci * es};
         // the whole tile (ht rows 2y + kh of nt images) as one box with traversal stride 2 along H (boxDim counts traversed
-        // elements: 2*ht -> ht rows); the per-row form remains for GIFB200_CONV_S2_ROWS=1 (A/B switch)
-        static const bool per_row = [] { const char* e = getenv("GIFB200_CONV_S2_ROWS"); return e && atoi(e) != 0; }();
-        const bool onebox = !per_row && p.ht * p.nt > 1;
-        if (onebox) p.s2 = 2;
-        const cuuint32_t box[5] = {kBlockK, 1, static_cast<cuuint32_t>(p.wt), static_cast<cuuint32_t>(onebox ? 2 * p.ht : 1),
-                                   static_cast<cuuint32_t>(onebox ? p.nt : 1)};
-        const cuuint32_t estr[5] = {1, 1, 1, static_cast<cuuint32_t>(onebox ? 2 : 1), 1};
+        // elements: 2*ht -> ht rows); a tile of one row (ht == nt == 1) takes a plain one-row box
+        const bool one_row = p.ht * p.nt == 1;
+        const cuuint32_t box[5] = {kBlockK, 1, static_cast<cuuint32_t>(p.wt), static_cast<cuuint32_t>(one_row ? 1 : 2 * p.ht),
+                                   static_cast<cuuint32_t>(p.nt)};
+        const cuuint32_t estr[5] = {1, 1, 1, static_cast<cuuint32_t>(one_row ? 1 : 2), 1};
         rc = encode_map(&ma, xb, 5, dims, strides, box, swz, dt, estr);
         if (rc == GIFB200_OK && x3) rc = encode_map(&ma2, xb + x_plane * es, 5, dims, strides, box, swz, dt, estr);
     }

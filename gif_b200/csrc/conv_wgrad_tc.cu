@@ -28,8 +28,6 @@
 // side CU_TENSOR_MAP_SWIZZLE_64B), which wgmma reads transposed; a stage holds the hi and the lo chunk set of each operand --
 // the SAME bytes as the fp32 tiles -- and every 16-pixel slice issues three bf16 wgmmas (lo*hi, hi*lo, hi*hi) per
 // warpgroup into the tap's fp32 accumulator.
-#include <stdlib.h>
-
 #include "tc_common.cuh"
 
 namespace gifb200 {
@@ -80,7 +78,7 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int ch) {
     return static_cast<uint32_t>(row * 128 + ((((ch >> 2) ^ row) & 7) << 4) + (ch & 3) * 4);
 }
 
-template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC, bool RS>
+template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC>
 __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_s,
                                                                  const __grid_constant__ CUtensorMap map_s2,
                                                                  const __grid_constant__ CUtensorMap map_b,
@@ -200,11 +198,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
             for (int i = 0; i < kAcc; ++i) acc[kw][i] = 0.f;
         int stage = 0, prev = -1;
         uint32_t ph = 0;
-        // RS: the A operand of a slice (this warpgroup's 64 rows x 16 pixels of S, hi and lo plane) is the same for all KW
-        // taps and for two of the three MMAs of each tap, so it is loaded into registers once per slice (ldmatrix .trans of
-        // the MN-major tile) and only B is read from shared memory by the wgmmas: half the operand bytes of SS.  The MMAs,
-        // their order and the accumulators are those of SS.  wgmma reads the fragments asynchronously and the previous
-        // stage's group is still in flight when the next stage loads its own, so the fragments alternate between two sets.
+        // The A operand of a slice (this warpgroup's 64 rows x 16 pixels of S, hi and lo plane) is the same for all KW taps
+        // and for two of the three MMAs of each tap, so it is loaded into registers once per slice (ldmatrix .trans of the
+        // MN-major tile) and only B is read from shared memory by the wgmmas.  wgmma reads the fragments asynchronously and
+        // the previous stage's group is still in flight when the next stage loads its own, so the fragments alternate
+        // between two sets.
         uint32_t afr[2][kSlices][2][4];      // [set][slice][plane: 0 = hi, 1 = lo][register]
         // this lane's ldmatrix row: matrix mi = lane / 8 covers rows +8 (mi & 1) and pixels +8 (mi >> 1) of the warp's 16 x 16
         // block, row r = lane % 8 is pixel r of it; a pixel row is 64 B and SWIZZLE_64B XORs its 16 B unit with (pixel / 2) % 4
@@ -214,16 +212,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
         auto run_stage = [&](uint32_t (&fr)[kSlices][2][4]) {
             mbar_wait(&full_bar[stage], ph);
             const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-            const uint32_t a_row = AC == 4 ? wg * 2 * kChunkBytes : 0;
-            const uint64_t adesc = make_smem_desc(a_addr + a_row, kChunkBytes, 512, 2);
-            const uint64_t adesc_lo = make_smem_desc(a_addr + L::kAPlaneBytes + a_row, kChunkBytes, 512, 2);
-            if constexpr (RS) {
 #pragma unroll
-                for (int jj = 0; jj < kSlices; ++jj) {
-                    const int j = AC == 4 ? jj : wg;
+            for (int jj = 0; jj < kSlices; ++jj) {
+                const int j = AC == 4 ? jj : wg;
 #pragma unroll
-                    for (int pl = 0; pl < 2; ++pl) ldmatrix_x4_trans(fr[jj][pl], a_addr + pl * L::kAPlaneBytes + a_lane + 1024 * j);
-                }
+                for (int pl = 0; pl < 2; ++pl) ldmatrix_x4_trans(fr[jj][pl], a_addr + pl * L::kAPlaneBytes + a_lane + 1024 * j);
             }
             wgmma_fence();
 #pragma unroll
@@ -239,15 +232,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
 #pragma unroll
                 for (int jj = 0; jj < kSlices; ++jj) {   // 16 pixels per MMA = two 8-pixel atoms: next slice = +1024 B (>>4 = 64)
                     const int j = AC == 4 ? jj : wg;
-                    if constexpr (RS) {
-                        wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][1], bdesc + 64 * j, 1, Trans<1>());
-                        wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][0], bdesc_lo + 64 * j, 1, Trans<1>());
-                        wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][0], bdesc + 64 * j, 1, Trans<1>());
-                    } else {
-                        wgmma_bf16<BLOCK_N>(acc[kw], adesc_lo + 64 * j, bdesc + 64 * j, 1, Trans<1>());
-                        wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc_lo + 64 * j, 1, Trans<1>());
-                        wgmma_bf16<BLOCK_N>(acc[kw], adesc + 64 * j, bdesc + 64 * j, 1, Trans<1>());
-                    }
+                    wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][1], bdesc + 64 * j, 1, Trans<1>());
+                    wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][0], bdesc_lo + 64 * j, 1, Trans<1>());
+                    wgmma_bf16_rs<BLOCK_N>(acc[kw], fr[jj][0], bdesc + 64 * j, 1, Trans<1>());
                 }
             }
             wgmma_commit();
@@ -258,13 +245,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_tc_kernel(const __grid_co
             prev = stage;
             if (++stage == kNStages) { stage = 0; ph ^= 1; }
         };
-        if constexpr (RS) {
-            for (int it = 0; it < iters; it += 2) {
-                run_stage(afr[0]);
-                if (it + 1 < iters) run_stage(afr[1]);
-            }
-        } else {
-            for (int it = 0; it < iters; ++it) run_stage(afr[0]);
+        for (int it = 0; it < iters; it += 2) {
+            run_stage(afr[0]);
+            if (it + 1 < iters) run_stage(afr[1]);
         }
         wgmma_wait<0>();
 #pragma unroll
@@ -402,17 +385,17 @@ int pick_bn(int Cb) {
 
 struct WgMaps { CUtensorMap s, s2, b, b2; };
 
-template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC, bool RS>
+template <int KW, int BLOCK_N, bool STACK, bool HALO, bool X3, int AC>
 int launch_wg(const WgMaps& m, float* out, float* part, const WgParams& p, cudaStream_t st) {
     using L = WgSmem<KW, BLOCK_N, HALO, X3, AC>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
+        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kDynamic);
         if (e != cudaSuccess) return fail(GIFB200_E_CUDA, "cudaFuncSetAttribute(wgrad_tc_kernel)", cudaGetErrorString(e));
         attr_set = true;
     }
     dim3 grid(STACK || AC == 2 ? 1 : p.Cs / 128, p.Cb / BLOCK_N, STACK ? p.splits : p.k * p.splits);
-    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC, RS><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
+    wgrad_tc_kernel<KW, BLOCK_N, STACK, HALO, X3, AC><<<grid, kWgThreads, L::kDynamic, st>>>(m.s, m.s2, m.b, m.b2, part, p);
     GIFB200_LAUNCH_CHECK("wgrad_tc_kernel");
     const int T = p.k * p.k;
     const long long total = static_cast<long long>(T) * p.Cs * p.Cb;
@@ -471,11 +454,11 @@ size_t conv2d_wgrad_tc_workspace_bytes(int B, int Hi, int Wi, int Ci, int Ho, in
     return static_cast<size_t>(wgrad_splits(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, nullptr)) * k * k * Co * Ci * sizeof(float) + 256;
 }
 
-template <bool X3, bool RS>
+template <bool X3>
 static int dispatch_wg(int k, int bn, bool stack, bool narrow, bool halo, const WgMaps& m, float* gw, float* part, const WgParams& p,
                        cudaStream_t st) {
-#define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3, 4, RS>(m, gw, part, p, st)
-#define GIFB200_WGN(KW, BN, HA) launch_wg<KW, BN, false, HA, X3, 2, RS>(m, gw, part, p, st)
+#define GIFB200_WG(KW, BN, ST, HA) launch_wg<KW, BN, ST, HA, X3, 4>(m, gw, part, p, st)
+#define GIFB200_WGN(KW, BN, HA) launch_wg<KW, BN, false, HA, X3, 2>(m, gw, part, p, st)
     if (narrow) {
         if (halo) return bn == 64 ? GIFB200_WGN(3, 64, true) : GIFB200_WGN(3, 32, true);
         if (k == 3) return bn == 64 ? GIFB200_WGN(3, 64, false) : GIFB200_WGN(3, 32, false);
@@ -540,9 +523,7 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
         if (rc == GIFB200_OK && x3) rc = encode_map(&m.s2, Sb + s_plane, 4, dims, strides, box, swz, dt);
         if (rc != GIFB200_OK) return rc;
     }
-    // GIFB200_WGRAD_HALO: 0 = off, 1 = on (default)
-    static const int halo_env = [] { const char* e = getenv("GIFB200_WGRAD_HALO"); return e ? atoi(e) : 1; }();
-    const bool halo = halo_env > 0 && mode == 0 && k == 3 && p.pw == kPix;
+    const bool halo = mode == 0 && k == 3 && p.pw == kPix;
     if (!p.s2) {
         const cuuint64_t dims[4] = {static_cast<cuuint64_t>(p.Cb), static_cast<cuuint64_t>(p.Wb), static_cast<cuuint64_t>(p.Hb), static_cast<cuuint64_t>(B)};
         const cuuint64_t strides[3] = {static_cast<cuuint64_t>(p.Cb) * es, static_cast<cuuint64_t>(p.Wb) * p.Cb * es,
@@ -569,12 +550,8 @@ int conv2d_wgrad_tc(const float* x, const float* gy, float* gw, int B, int Hi, i
         if (rc != GIFB200_OK) return rc;
     }
     if (!x3) { m.s2 = m.s; m.b2 = m.b; }
-    if (!x3) return dispatch_wg<false, false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
-    // GIFB200_WGRAD_X3_RS: 1 = the bf16x3 wgmmas take the S operand from registers (default), 0 = from shared memory like B.
-    // Both issue the same MMAs in the same order into the same accumulators: the results are bitwise the same.
-    static const int rs_env = [] { const char* e = getenv("GIFB200_WGRAD_X3_RS"); return e ? atoi(e) : 1; }();
-    return rs_env > 0 ? dispatch_wg<true, true>(k, bn, stack, narrow, halo, m, gw, part, p, st)
-                      : dispatch_wg<true, false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
+    return x3 ? dispatch_wg<true>(k, bn, stack, narrow, halo, m, gw, part, p, st)
+              : dispatch_wg<false>(k, bn, stack, narrow, halo, m, gw, part, p, st);
 }
 
 }  // namespace gifb200

@@ -10,7 +10,6 @@ Conventions
   * there is no CPU / eager fallback: non-CUDA tensors raise.
 """
 import math
-import os
 import weakref
 
 import torch
@@ -370,7 +369,7 @@ def conv2d(x, w, k, mode=S1, flip=False, transposed=False):
     return _Conv.apply(x, w, k, mode, flip, transposed, (conv_out_size(hi, k, mode), conv_out_size(wi, k, mode)))
 
 
-_NO_WEIGHT_CACHE = bool(os.environ.get("GIFB200_NO_WEIGHT_CACHE"))    # A/B switch: recompute the tap-major weights on every call
+_NO_WEIGHT_CACHE = False    # tests set this to compare against prepare-and-stage on every call (as cache=False)
 _prep_cache = {}     # (id of the parameter, view offset, shape, scale) -> (weakref to the parameter, its version, buffer, serial,
                      #                                                  address of the weight)
 _stage_cache = {}    # (prep key, flip, transposed, impl, conv shape) -> [prep serial it was staged from, persistent workspace]

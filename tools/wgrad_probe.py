@@ -2,18 +2,12 @@
 """Single weight-gradient launches through the C ABI for timing.
 
     python tools/wgrad_probe.py [ns|mid|low|s2|t2] ...              tf32 kernel on the named shapes
-    python tools/wgrad_probe.py --precision bf16x3 [--rounds R] [name ...]
-                                                                    bf16x3 kernel on the 256^2 step's weight-gradient shapes: both
-                                                                    operands from shared memory and one B tile per tap
-                                                                    (GIFB200_WGRAD_X3_RS=0 GIFB200_WGRAD_HALO=0, "ss") and the
-                                                                    default (S operand in registers, halo tile: "rs"), alternating
-                                                                    for R rounds (one child process per path and round: the
-                                                                    switches are read once)
+    python tools/wgrad_probe.py --precision bf16x3 [name ...]       bf16x3 kernel on the 256^2 step's weight-gradient shapes
+
+To compare two builds, run the tool in each checkout.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -74,14 +68,14 @@ def tf32_main(names):
         print(f"{n}: {ms:.3f} ms  {_tflops(mode, b, r, ci, co, 3, ms):.1f} TFLOP/s", flush=True)
 
 
-def x3_child(names):
-    """One path (whatever GIFB200_WGRAD_X3_RS says): {name: ms} of the bf16x3 weight gradient on the split planes."""
+def x3_main(names):
+    """ms and algorithmic TFLOP/s of the bf16x3 weight gradient on the split planes of each named shape."""
     import torch
     from gif_b200 import ops
     from gif_b200._lib import lib
     dev = torch.device("cuda:0")
     ops.set_precision("bf16x3")
-    out = {}
+    print(f"{'shape':<14} {'ms':>8} {'TFLOP/s':>8}")
     for n in names:
         mode, b, r, ci, co, k = X3_CASES[n]
         mode = getattr(ops, mode)
@@ -90,41 +84,18 @@ def x3_child(names):
         x = torch.randn(b, r, r, ci, device=dev)
         gy = torch.randn(b, ho, ho, co, device=dev)
         xp, gp = ops._planes(x), ops._planes(gy)                # split once: time the weight gradient alone
-        out[n] = _time(lambda: ops._wgrad_raw(x, gy, k, mode, False, False, x_planes=xp))
+        ms = _time(lambda: ops._wgrad_raw(x, gy, k, mode, False, False, x_planes=xp))
+        print(f"{n:<14} {ms:8.3f} {_tflops(mode, b, r, ci, co, k, ms):8.1f}", flush=True)
         del x, gy, xp, gp
         torch.cuda.empty_cache()
-    print(json.dumps(out), flush=True)
-
-
-def x3_main(names, rounds):
-    runs = {"ss": [], "rs": []}
-    for _ in range(rounds):
-        for path, rs in (("ss", "0"), ("rs", "1")):
-            r = subprocess.run([sys.executable, os.path.abspath(__file__), "--x3-child"] + names,
-                               env=dict(os.environ, GIFB200_WGRAD_X3_RS=rs, GIFB200_WGRAD_HALO=rs), capture_output=True, text=True)
-            if r.returncode != 0:
-                sys.exit(r.stdout + r.stderr)
-            runs[path].append(json.loads(r.stdout.strip().splitlines()[-1]))
-    print(f"{'shape':<14} {'ss ms (min-max)':>17} {'rs ms (min-max)':>17} {'ss TFLOP/s':>11} {'rs TFLOP/s':>11} {'speed-up':>8}")
-    for n in names:
-        mode, b, r, ci, co, k = X3_CASES[n]
-        ss, rs = [x[n] for x in runs["ss"]], [x[n] for x in runs["rs"]]
-        from gif_b200 import ops
-        m = getattr(ops, mode)
-        print(f"{n:<14} {min(ss):7.3f}-{max(ss):7.3f}   {min(rs):7.3f}-{max(rs):7.3f}   {_tflops(m, b, r, ci, co, k, min(ss)):9.1f}  "
-              f"{_tflops(m, b, r, ci, co, k, min(rs)):9.1f}  {min(ss) / min(rs):7.3f}x", flush=True)
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--precision", default="tf32", choices=["tf32", "bf16x3"])
-    ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--x3-child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("names", nargs="*")
     a = ap.parse_args()
-    if a.x3_child:
-        x3_child(a.names)
-    elif a.precision == "bf16x3":
-        x3_main(a.names or list(X3_CASES), a.rounds)
+    if a.precision == "bf16x3":
+        x3_main(a.names or list(X3_CASES))
     else:
         tf32_main(a.names or list(CASES))
