@@ -74,6 +74,9 @@ SIGNATURES = {
     "gifb200_resize_bicubic_u8": (_i, [_p] * 5 + [_i] * 7 + [_p]),
     "gifb200_u8_to_unit": (_i, [_p, _p, _i, _i, _i, _ll, _p]),
     "gifb200_image_to_u8": (_i, [_p, _p, _i, _i, _i, _ll, _ll, _ll, _ll, _p]),
+    "gifb200_jpeg_encode_workspace_bytes": (_sz, [_i, _i, _i]),
+    "gifb200_jpeg_encode_out_bytes": (_sz, [_i, _i, _i]),
+    "gifb200_jpeg_encode": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _sz, _p]),
 }
 
 

@@ -13,7 +13,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libgifb200.so")
-SOURCES = ["elementwise.cu", "optim.cu", "upfirdn2d.cu", "sgemm.cu", "conv_simt.cu", "conv_tc.cu", "conv_wgrad_tc.cu", "conv_api.cu", "conv_ex.cu", "pool_resize.cu", "rasterize.cu", "render.cu", "flame.cu", "texture.cu", "image_decode.cu"]
+SOURCES = ["elementwise.cu", "optim.cu", "upfirdn2d.cu", "sgemm.cu", "conv_simt.cu", "conv_tc.cu", "conv_wgrad_tc.cu", "conv_api.cu", "conv_ex.cu", "pool_resize.cu", "rasterize.cu", "render.cu", "flame.cu", "texture.cu", "image_decode.cu", "jpeg_encode.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
          "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]

@@ -447,13 +447,23 @@ extern "C" int gifb200_png_unfilter(uint8_t* data, const int32_t* desc, int n_im
 
 extern "C" int gifb200_resize_bicubic_u8(const uint8_t* x, uint8_t* tmp, uint8_t* y, const int32_t* coef_h, const int32_t* coef_v,
                                          int B, int Hi, int Wi, int Ho, int Wo, int ks_h, int ks_v, gifb200_stream_t stream) {
-    GIFB200_REQUIRE(B > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0 && ks_h > 0 && ks_v > 0, GIFB200_E_SHAPE,
-                    "resize_bicubic_u8: positive sizes and tap counts");
+    GIFB200_REQUIRE(B > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0, GIFB200_E_SHAPE, "resize_bicubic_u8: positive sizes");
+    GIFB200_REQUIRE((coef_h ? ks_h > 0 : Wo == Wi) && (coef_v ? ks_v > 0 : Ho == Hi) && (tmp || !coef_h || !coef_v),
+                    GIFB200_E_SHAPE, "resize_bicubic_u8: a skipped pass keeps its axis; a pass needs taps; two passes need tmp");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    resize_h_kernel<<<grid_for(static_cast<long long>(B) * Hi * Wo), 256, 0, st>>>(x, tmp, coef_h, B, Hi, Wi, Wo, ks_h);
-    GIFB200_LAUNCH_CHECK("resize_h_kernel");
-    resize_v_kernel<<<grid_for(static_cast<long long>(B) * Ho * Wo), 256, 0, st>>>(tmp, y, coef_v, B, Hi, Ho, Wo, ks_v);
-    GIFB200_LAUNCH_CHECK("resize_v_kernel");
+    if (!coef_h && !coef_v) {
+        if (cudaMemcpyAsync(y, x, 3ull * B * Hi * Wi, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+            return fail(GIFB200_E_CUDA, "resize_bicubic_u8: cudaMemcpyAsync", cudaGetErrorString(cudaGetLastError()));
+        return GIFB200_OK;
+    }
+    if (coef_h) {
+        resize_h_kernel<<<grid_for(static_cast<long long>(B) * Hi * Wo), 256, 0, st>>>(x, coef_v ? tmp : y, coef_h, B, Hi, Wi, Wo, ks_h);
+        GIFB200_LAUNCH_CHECK("resize_h_kernel");
+    }
+    if (coef_v) {
+        resize_v_kernel<<<grid_for(static_cast<long long>(B) * Ho * Wo), 256, 0, st>>>(coef_h ? tmp : x, y, coef_v, B, Hi, Ho, Wo, ks_v);
+        GIFB200_LAUNCH_CHECK("resize_v_kernel");
+    }
     return GIFB200_OK;
 }
 

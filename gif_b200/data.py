@@ -15,8 +15,9 @@ dataset_loaders.py:128-137) and returns ``(img, [cat(render, normal)], [flame_la
 This module reads that format WITHOUT the ``lmdb`` package (absent from the image; a dependency of the reference, not a
 vendored source): ``LmdbReader`` is a read-only walker of LMDB's published file format (data.mdb: two meta pages, a B+tree of
 branch / leaf pages with 2-byte node offsets, overflow pages for values larger than half a page), restated from the format
-description in lmdb's mdb.c / lmdb.h (MDB_page, MDB_node, MDB_meta, MDB_db).  ``write_lmdb`` is a bulk writer of the same
-format used to build fixtures (sorted keys -> packed leaves -> branch levels -> meta pages).  PARITY UNPINNED: no LMDB file and
+description in lmdb's mdb.c / lmdb.h (MDB_page, MDB_node, MDB_meta, MDB_db).  ``LmdbWriter`` is a streaming bulk writer of the
+same format (overflow values appended as they arrive; packed leaves -> branch levels -> meta pages at the end) and
+``write_lmdb`` its sorted-input form for fixtures.  PARITY UNPINNED: no LMDB file and
 no lmdb library exist here to check either against; reader and writer are tested against each other and against the
 documented layout constants (tests/test_data_cpu.py).
 
@@ -165,38 +166,65 @@ class LmdbReader:
             yield from walk(self.meta["root"])
 
 
-def write_lmdb(path, items, page_size=4096):
-    """Bulk-write ``items`` (an iterable of (key bytes, value bytes)) as an LMDB environment directory ``path`` (data.mdb).
-    Packed leaves, branch levels built bottom-up, values that do not fit half a page go to overflow pages -- the layout a
-    reader of the published format (and ``LmdbReader``) expects.  Fixture / export tool, not a transactional store."""
-    items = sorted((k if isinstance(k, bytes) else k.encode("utf-8"), bytes(v)) for k, v in items)
-    for (a, _), (b, _) in zip(items, items[1:]):
-        if a == b:
-            raise ValueError(f"duplicate key {a!r}")
-    os.makedirs(path, exist_ok=True)
-    node_max = ((page_size - PAGE_HDR) // 2 - 2) & ~1            # mdb.c: me_nodemax
-    pages = {}                                                     # pgno -> bytes
-    next_pg = [2]
+class LmdbWriter:
+    """Streaming bulk writer of an LMDB environment directory ``path`` (data.mdb) in the layout ``LmdbReader`` and readers
+    of the published format expect: packed leaves, branch levels built bottom-up, values that do not fit half a page in
+    overflow pages.  Values may arrive in any order (LMDB pages have no sibling links): ``put`` appends a large value's
+    overflow pages to the file at once and keeps only small values and (key, first page, size) in memory; ``close`` sorts
+    the keys and writes the leaves, the branch levels and the two meta pages.  A multiscale image set of ~100 GB therefore
+    never sits in memory.  Fixture / export tool, not a transactional store: the file is complete only after ``close``."""
 
-    def alloc(n=1):
-        p = next_pg[0]
-        next_pg[0] += n
-        return p
+    def __init__(self, path, page_size=4096):
+        os.makedirs(path, exist_ok=True)
+        self.path = os.path.join(path, "data.mdb")
+        self.page_size = page_size
+        self.node_max = ((page_size - PAGE_HDR) // 2 - 2) & ~1        # mdb.c: me_nodemax
+        self.entries = []                                                # (key, node payload, node flags, data size)
+        self.overflow_pages = 0
+        self.next_pg = 2
+        self.f = open(self.path, "wb")
+        self.f.write(bytes(2 * page_size))                               # the meta pages, written last
 
-    def even(n):
-        return (n + 1) & ~1
+    def __enter__(self):
+        return self
 
-    def build_level(entries, leaf):
-        """entries: leaf -> (key, node payload bytes, node flags, data size); branch -> (key, child pgno).  Returns
-        [(first key, pgno)] of the pages written."""
+    def __exit__(self, exc_type, *_):
+        if exc_type is None:
+            self.close()
+        else:
+            self.f.close()
+
+    def put(self, key, value):
+        key = key if isinstance(key, bytes) else key.encode("utf-8")
+        value = bytes(value)
+        if len(key) > 511:
+            raise ValueError("LMDB keys are at most 511 bytes")
+        if NODE_HDR + len(key) + len(value) > self.node_max:
+            n = (PAGE_HDR + len(value) + self.page_size - 1) // self.page_size
+            pg = self.next_pg
+            self.next_pg += n
+            self.f.write(struct.pack("<QHHI", pg, 0, P_OVERFLOW, n) + value + bytes(n * self.page_size - PAGE_HDR - len(value)))
+            self.overflow_pages += n
+            self.entries.append((key, struct.pack("<Q", pg), F_BIGDATA, len(value)))
+        else:
+            self.entries.append((key, value, 0, len(value)))
+
+    def _level(self, entries, leaf):
+        """Write one tree level.  entries: leaf -> (key, node payload, node flags, data size); branch -> (key, child pgno).
+        Returns [(first key, pgno)] of the pages written."""
         out, cur, used = [], [], 0
+        page_size = self.page_size
         cap = page_size - PAGE_HDR
+
+        def even(n):
+            return (n + 1) & ~1
 
         def flush():
             nonlocal cur, used
             if not cur:
                 return
-            pgno = alloc()
+            pgno = self.next_pg
+            self.next_pg += 1
             page = bytearray(page_size)
             upper = page_size
             ptrs = []
@@ -217,55 +245,58 @@ def write_lmdb(path, items, page_size=4096):
             assert lower <= upper
             struct.pack_into("<QHHHH", page, 0, pgno, 0, P_LEAF if leaf else P_BRANCH, lower, upper)
             struct.pack_into(f"<{len(ptrs)}H", page, PAGE_HDR, *ptrs)
-            pages[pgno] = bytes(page)
+            self.f.write(page)
             out.append((cur[0][0], pgno))
             cur, used = [], 0
         for e in entries:
-            ksz = len(e[0])
-            nsz = even(NODE_HDR + ksz + (len(e[1]) if leaf else 0)) + 2
+            nsz = even(NODE_HDR + len(e[0]) + (len(e[1]) if leaf else 0)) + 2
             if used + nsz > cap:
                 flush()
             cur.append(e)
             used += nsz
         flush()
         return out
-    leaf_entries, overflow_pages = [], 0
-    for k, v in items:
-        if len(k) > 511:
-            raise ValueError("LMDB keys are at most 511 bytes")
-        if NODE_HDR + len(k) + len(v) > node_max:
-            n = (PAGE_HDR + len(v) + page_size - 1) // page_size
-            pg = alloc(n)
-            blob = bytearray(n * page_size)
-            struct.pack_into("<QHHI", blob, 0, pg, 0, P_OVERFLOW, n)
-            blob[PAGE_HDR:PAGE_HDR + len(v)] = v
-            for j in range(n):
-                pages[pg + j] = bytes(blob[j * page_size:(j + 1) * page_size])
-            overflow_pages += n
-            leaf_entries.append((k, struct.pack("<Q", pg), F_BIGDATA, len(v)))
-        else:
-            leaf_entries.append((k, v, 0, len(v)))
-    level = build_level(leaf_entries, True)
-    leaf_pages, branch_pages, depth = len(level), 0, 1 if level else 0
-    while len(level) > 1:
-        level = build_level(level, False)
-        branch_pages += len(level)
-        depth += 1
-    root = level[0][1] if level else P_INVALID
-    last_pg = next_pg[0] - 1
-    with open(os.path.join(path, "data.mdb"), "wb") as f:
+
+    def close(self):
+        """Sort the keys, write the tree and the meta pages; returns the path of data.mdb."""
+        entries = sorted(self.entries, key=lambda e: e[0])
+        for a, b in zip(entries, entries[1:]):
+            if a[0] == b[0]:
+                self.f.close()
+                raise ValueError(f"duplicate key {a[0]!r}")
+        level = self._level(entries, True)
+        leaf_pages, branch_pages, depth = len(level), 0, 1 if level else 0
+        while len(level) > 1:
+            level = self._level(level, False)
+            branch_pages += len(level)
+            depth += 1
+        root = level[0][1] if level else P_INVALID
+        last_pg = self.next_pg - 1
+        self.f.seek(0)
         for pg in (0, 1):
-            page = bytearray(page_size)
+            page = bytearray(self.page_size)
             struct.pack_into("<QHHHH", page, 0, pg, 0, P_META, 0, 0)
-            free_db = struct.pack("<IHHQQQQQ", page_size, 0, 0, 0, 0, 0, 0, P_INVALID)
-            main_db = struct.pack("<IHHQQQQQ", 0, 0, depth, branch_pages, leaf_pages, overflow_pages, len(items), root)
-            meta = struct.pack("<IIQQ", MDB_MAGIC, MDB_VERSION, 0, max(1 << 20, (last_pg + 1) * page_size)) + free_db + main_db + \
-                struct.pack("<QQ", last_pg, pg)                    # txnid: page 1 is the newer one
+            free_db = struct.pack("<IHHQQQQQ", self.page_size, 0, 0, 0, 0, 0, 0, P_INVALID)
+            main_db = struct.pack("<IHHQQQQQ", 0, 0, depth, branch_pages, leaf_pages, self.overflow_pages, len(entries), root)
+            meta = struct.pack("<IIQQ", MDB_MAGIC, MDB_VERSION, 0, max(1 << 20, (last_pg + 1) * self.page_size)) + free_db + \
+                main_db + struct.pack("<QQ", last_pg, pg)              # txnid: page 1 is the newer one
             page[PAGE_HDR:PAGE_HDR + len(meta)] = meta
-            f.write(page)
-        for pg in range(2, last_pg + 1):
-            f.write(pages[pg])
-    return os.path.join(path, "data.mdb")
+            self.f.write(page)
+        self.f.close()
+        return self.path
+
+
+def write_lmdb(path, items, page_size=4096):
+    """Bulk-write ``items`` (an iterable of (key bytes, value bytes)) as an LMDB environment directory ``path`` (data.mdb),
+    through ``LmdbWriter`` in key order.  Returns the path of data.mdb."""
+    items = sorted((k if isinstance(k, bytes) else k.encode("utf-8"), bytes(v)) for k, v in items)
+    for (a, _), (b, _) in zip(items, items[1:]):
+        if a == b:
+            raise ValueError(f"duplicate key {a!r}")
+    w = LmdbWriter(path, page_size)
+    for k, v in items:
+        w.put(k, v)
+    return w.close()
 
 
 # ---------------------------------------------------------------------------------------------- key schema / decode

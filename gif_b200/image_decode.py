@@ -7,11 +7,12 @@ costs one host-to-device copy; ``decode_*`` then run the kernels of csrc/image_d
 
     JPEG  parallel entropy decode -> dequantise + islow IDCT -> fancy upsampling + YCbCr->RGB       (libjpeg-turbo defaults)
     PNG   scanline unfiltering (None/Sub/Up/Average/Paeth) -> RGB (grey replicated, alpha dropped)  (``convert("RGB")``)
-    resize Pillow's two-pass bicubic with 22-bit fixed-point weights                                  (``Image.resize``)
+    resize Pillow's two-pass bicubic / Lanczos with 22-bit fixed-point weights                        (``Image.resize``)
     unit  (v / 255 - 0.5) / 0.5 into NCHW slices                                                      (ToTensor + Normalize)
 
 Anything outside the supported subset raises ``UnsupportedImage`` naming the reason; ``data.decode_image`` (PIL) remains
 the path for such files."""
+import math
 import re
 import struct
 import zlib
@@ -426,13 +427,24 @@ def _bicubic(x):
     return 0.0
 
 
-@lru_cache(maxsize=64)
-def bicubic_coeffs(in_size, out_size):
-    """Pillow's precompute_coeffs + normalize_coeffs_8bpc for the bicubic filter (support 2, widened by the scale when
-    downscaling), in float64: int32 (out_size, ks + 2) rows [first tap, tap count, 22-bit weights...]."""
+def _sinc(x):
+    if x == 0.0:
+        return 1.0
+    x = x * math.pi
+    return math.sin(x) / x
+
+
+def _lanczos(x):
+    """Pillow's truncated sinc (lanczos_filter), through the C library's sin as Pillow calls it, one value at a time."""
+    return _sinc(x) * _sinc(x / 3) if -3.0 <= x < 3.0 else 0.0
+
+
+def _resample_coeffs(filt, support, in_size, out_size):
+    """Pillow's precompute_coeffs + normalize_coeffs_8bpc (the filter's support widened by the scale when downscaling), in
+    float64: int32 (out_size, ks + 2) rows [first tap, tap count, 22-bit weights...]."""
     scale = in_size / out_size
     fscale = max(scale, 1.0)
-    support = 2.0 * fscale
+    support = support * fscale
     ks = int(np.ceil(support)) * 2 + 1
     out = np.zeros((out_size, ks + 2), np.int32)
     for xx in range(out_size):
@@ -440,7 +452,7 @@ def bicubic_coeffs(in_size, out_size):
         ss = 1.0 / fscale
         xmin = max(int(center - support + 0.5), 0)
         xmax = min(int(center + support + 0.5), in_size) - xmin
-        w = [_bicubic((x + xmin - center + 0.5) * ss) for x in range(xmax)]
+        w = [filt((x + xmin - center + 0.5) * ss) for x in range(xmax)]
         tot = sum(w)
         w = [v / tot if tot != 0.0 else v for v in w]
         out[xx, 0], out[xx, 1] = xmin, xmax
@@ -450,26 +462,65 @@ def bicubic_coeffs(in_size, out_size):
 
 
 @lru_cache(maxsize=64)
-def _bicubic_coeffs_device(W, H, size, device):
-    """``bicubic_coeffs`` of both passes on the device, uploaded once per shape: a per-call upload would wait for the
-    stream (a blocking host-to-device copy) and stall a pipeline that keeps the device busy."""
-    ch, cv = bicubic_coeffs(W, size), bicubic_coeffs(H, size)
-    return torch.from_numpy(np.concatenate([ch.ravel(), cv.ravel()])).to(device), ch.size, ch.shape[1] - 2, cv.shape[1] - 2
+def bicubic_coeffs(in_size, out_size):
+    """``_resample_coeffs`` of Pillow's bicubic filter (support 2)."""
+    return _resample_coeffs(_bicubic, 2.0, in_size, out_size)
+
+
+@lru_cache(maxsize=64)
+def lanczos_coeffs(in_size, out_size):
+    """``_resample_coeffs`` of Pillow's Lanczos filter (support 3)."""
+    return _resample_coeffs(_lanczos, 3.0, in_size, out_size)
+
+
+@lru_cache(maxsize=64)
+def _coeffs_device(coeffs, W, H, Wo, Ho, device):
+    """Both passes' coefficients on the device, uploaded once per shape: a per-call upload would wait for the stream (a
+    blocking host-to-device copy) and stall a pipeline that keeps the device busy.  A pass whose axis keeps its size is
+    skipped, as Pillow skips it: its table is empty and its tap count 0."""
+    ch = coeffs(W, Wo) if W != Wo else np.zeros((0, 2), np.int32)
+    cv = coeffs(H, Ho) if H != Ho else np.zeros((0, 2), np.int32)
+    t = torch.from_numpy(np.concatenate([ch.ravel(), cv.ravel(), [0]]).astype(np.int32)).to(device)
+    return t, ch.size, ch.shape[1] - 2, cv.shape[1] - 2
+
+
+def _resize_u8(coeffs, x, Ho, Wo, tmp, out, name):
+    squeeze = x.dim() == 3
+    xb = x.unsqueeze(0) if squeeze else x
+    B, H, W, _ = xb.shape
+    coef, n_h, ks_h, ks_v = _coeffs_device(coeffs, W, H, Wo, Ho, x.device)
+    if tmp is None and ks_h and ks_v:
+        tmp = torch.empty(B, H, Wo, 3, dtype=torch.uint8, device=x.device)
+    out = torch.empty(B, Ho, Wo, 3, dtype=torch.uint8, device=x.device) if out is None else out
+    _lib.check(_lib.lib.gifb200_resize_bicubic_u8(xb.contiguous().data_ptr(), tmp.data_ptr() if tmp is not None else None,
+                                                  out.data_ptr(), coef.data_ptr() if ks_h else None,
+                                                  coef.data_ptr() + 4 * n_h if ks_v else None, B, H, W, Ho, Wo, ks_h, ks_v,
+                                                  _lib.stream()), name)
+    return out[0] if squeeze else out
 
 
 def resize_bicubic_u8(x, size, tmp=None, out=None):
     """uint8 (B, H, W, 3) or (H, W, 3) CUDA tensor -> (B, size, size, 3): Pillow's ``Image.resize((size, size))`` (bicubic),
     bit for bit."""
-    squeeze = x.dim() == 3
-    xb = x.unsqueeze(0) if squeeze else x
-    B, H, W, _ = xb.shape
-    coef, n_h, ks_h, ks_v = _bicubic_coeffs_device(W, H, size, x.device)
-    tmp = torch.empty(B, H, size, 3, dtype=torch.uint8, device=x.device) if tmp is None else tmp
-    out = torch.empty(B, size, size, 3, dtype=torch.uint8, device=x.device) if out is None else out
-    _lib.check(_lib.lib.gifb200_resize_bicubic_u8(xb.contiguous().data_ptr(), tmp.data_ptr(), out.data_ptr(), coef.data_ptr(),
-                                                  coef.data_ptr() + 4 * n_h, B, H, W, size, size, ks_h, ks_v, _lib.stream()),
-               "resize_bicubic_u8")
-    return out[0] if squeeze else out
+    return _resize_u8(bicubic_coeffs, x, size, size, tmp, out, "resize_bicubic_u8")
+
+
+def resize_lanczos_u8(x, size, tmp=None, out=None):
+    """uint8 (B, H, W, 3) or (H, W, 3) CUDA tensor -> (B, Ho, Wo, 3) for ``size`` = (Ho, Wo): Pillow's
+    ``Image.resize((Wo, Ho), Image.LANCZOS)``, bit for bit."""
+    Ho, Wo = size
+    return _resize_u8(lanczos_coeffs, x, Ho, Wo, tmp, out, "resize_lanczos_u8")
+
+
+def resized_crop_box(w, h, size):
+    """torchvision's ``resize(img, size)`` (an int: the short side becomes ``size``, the long side ``int(size * long /
+    short)``; an image already of that size is left alone) then ``center_crop(size)``, for a PIL image of w x h:
+    ((resized w, resized h), (left, top)) of the crop.  Rounding of the offset is Python's (halves to even), as there."""
+    if w <= h:
+        rw, rh = size, int(size * h / w)
+    else:
+        rw, rh = int(size * w / h), size
+    return (rw, rh), (int(round((rw - size) / 2.0)), int(round((rh - size) / 2.0)))
 
 
 def u8_to_unit(x, out):

@@ -380,7 +380,9 @@ int gifb200_png_unfilter(uint8_t* data, const int32_t* desc, int n_img, int max_
 
 /* Pillow's Image.resize((Wo, Ho)) of uint8 RGB images (B, Hi, Wi, 3) -> (B, Ho, Wo, 3): horizontal pass into tmp
  * (B, Hi, Wo, 3), then vertical.  coef_h (Wo x (ks_h + 2)) / coef_v (Ho x (ks_v + 2)) rows = [first tap, tap count,
- * 22-bit fixed-point weights], computed by the host in float64 as Pillow's precompute_coeffs does. */
+ * 22-bit fixed-point weights], computed by the host in float64 as Pillow's precompute_coeffs does, for any filter
+ * (bicubic, Lanczos).  A NULL coef_h / coef_v skips that pass, as Pillow does when the axis keeps its size (then tmp may
+ * be NULL; both NULL copies x). */
 int gifb200_resize_bicubic_u8(const uint8_t* x, uint8_t* tmp, uint8_t* y, const int32_t* coef_h, const int32_t* coef_v, int B,
                               int Hi, int Wi, int Ho, int Wo, int ks_h, int ks_v, gifb200_stream_t stream);
 
@@ -394,6 +396,18 @@ int gifb200_u8_to_unit(const uint8_t* x, float* y, int B, int H, int W, long lon
  * view of channels-last storage is read in place); y: dense uint8 (B, H, W, 3).  NaN inputs are outside the contract. */
 int gifb200_image_to_u8(const float* x, uint8_t* y, int B, int H, int W, long long stride_b, long long stride_c,
                         long long stride_h, long long stride_w, gifb200_stream_t stream);
+
+/* Baseline JPEG encoding of uint8 RGB images x (B, H, W, 3), one size per call, as Pillow's save(format="JPEG", quality=q)
+ * writes them (libjpeg-turbo defaults: 4:2:0, islow FDCT, Annex K Huffman tables, no restart interval): RGB->YCbCr,
+ * h2v2 downsampling, FDCT, quantisation, Huffman coding, padding with 1-bits and 0xFF00 byte stuffing.  tables: the int32
+ * tables of gif_b200/image_encode.encoder_tables(q) (quantisation reciprocals, then the DC0/AC0/DC1/AC1 code tables).
+ * out (at least gifb200_jpeg_encode_out_bytes): the entropy-coded bytes of the images back to back; sizes (B, int64):
+ * their byte counts.  The host adds the headers and EOI.  Bit offsets within an image are 32-bit, which bounds the size
+ * (both query functions return 0 outside it). */
+size_t gifb200_jpeg_encode_workspace_bytes(int B, int H, int W);
+size_t gifb200_jpeg_encode_out_bytes(int B, int H, int W);
+int gifb200_jpeg_encode(const uint8_t* x, const int32_t* tables, int B, int H, int W, uint8_t* out, long long* sizes, void* ws,
+                        size_t ws_bytes, gifb200_stream_t stream);
 
 #ifdef __cplusplus
 }
