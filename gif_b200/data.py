@@ -402,8 +402,8 @@ class DeviceBatchLoader:
     with the same order, seed handling and drop_last.  Real images must be baseline JPEG and renders 8-bit PNG, as the
     reference's LMDB writers store them; anything else raises ``UnsupportedImage`` naming the key.
 
-    A background thread reads the raw LMDB values, parses them, inflates the PNGs on a small thread pool and fills a pinned
-    byte arena.  The consuming thread enqueues one non-blocking copy of the arena plus the decode kernels on a side stream,
+    A background thread reads the raw LMDB values, parses them, inflates the PNGs on a small thread pool and packs them as
+    one ``image_decode.DecodeBatch`` (a pinned byte arena).  The consuming thread enqueues its decode on a side stream,
     one batch ahead, so batch k+1 decodes while the caller trains on batch k.  It yields device tensors (real (B,3,R,R),
     cond (B,6,R,R), labels (B,P), indices (B,) int64) -- the arguments of ``GifTrainer.train_iteration`` -- after making the
     current stream wait for their decode.  Each batch stays valid until the next one is requested.  Before yielding a batch
@@ -431,68 +431,43 @@ class DeviceBatchLoader:
         self.pin = torch.cuda.is_available()
         self._stream = None
 
-    def _host_batch(self, ids, pool):
+    def host_batch(self, ids, pool):
+        """The host side of one batch, run on the loader's thread: the LMDB reads, the JPEG parsing and, on ``pool``, the PNG
+        inflate, packed as one ``image_decode.DecodeBatch`` (real images, then renders, then normal maps); the labels,
+        indices and, when rendering, the raw parameter rows.  Real images must be JPEG at the dataset's resolution and
+        renders PNG at its rend_flm_res."""
         from . import image_decode as I
         ds, R, rr = self.ds, self.ds.resolution, self.ds.rend_flm_res
-        keys = [image_key(R, i) for i in ids]
         render = self.conditions is not None
-        rkeys = [] if render else [image_key(rr, i) for i in ids] + [normal_map_key(rr, i) for i in ids]
 
-        def png(k):
-            try:
-                h = I.parse_png(ds.rend.get(k))
-                if (h[0], h[1]) != (rr, rr):
-                    raise I.UnsupportedImage(f"{h[0]}x{h[1]} render, rend_flm_res is {rr}")
-                return h, I.inflate_png(h)
-            except I.UnsupportedImage as e:
-                raise I.UnsupportedImage(f"{k.decode()}: {e}") from None
-        pngs = pool.map(png, rkeys)                 # inflates on the pool while this thread parses the JPEGs (if any)
-        parsed = []
-        for k in keys:
-            try:
-                p = I.parse_jpeg(ds.real.get(k))
-            except I.UnsupportedImage as e:
-                raise I.UnsupportedImage(f"{k.decode()}: {e}") from None
-            if (p["w"], p["h"]) != (R, R):
-                raise I.UnsupportedImage(f"{k.decode()}: {p['w']}x{p['h']} real image, the dataset's resolution is {R}")
-            parsed.append(p)
-        pngs = list(pngs)
-        jb = I.JpegBatch(parsed)
-        pb = None if render else I.PngBatch([h for h, _ in pngs], [r for _, r in pngs])
-        sizes = [len(jb.data), 0 if render else pb.data_bytes, 4 * jb.ints.size, 0 if render else 4 * pb.desc.size]
-        offs = np.concatenate([[0], np.cumsum([(s + 255) // 256 * 256 for s in sizes])])
-        arena = torch.empty(int(offs[-1]), dtype=torch.uint8, pin_memory=self.pin)
-        a = arena.numpy()
-        a[:sizes[0]] = np.frombuffer(jb.data, np.uint8)
-        o = offs[1]
-        for _, r in pngs:
-            a[o:o + len(r)] = np.frombuffer(r, np.uint8)
-            o += len(r)
-        a[offs[2]:offs[2] + sizes[2]] = jb.ints.view(np.uint8)
-        if not render:
-            a[offs[3]:offs[3] + sizes[3]] = pb.desc.ravel().view(np.uint8)
+        def load(db, key, kind, size):
+            im = I.host_decode(db.get(key), key.decode())
+            if im.kind != kind or (im.w, im.h) != (size, size):
+                raise I.UnsupportedImage(f"{im.name}: a {im.w}x{im.h} {im.kind.upper()}; the dataset's "
+                                         f"{'renders' if kind == 'png' else 'real images'} are {size}x{size} {kind.upper()}s")
+            return im
+        rkeys = [] if render else [image_key(rr, i) for i in ids] + [normal_map_key(rr, i) for i in ids]
+        pngs = pool.map(lambda k: load(ds.rend, k, "png", rr), rkeys)   # inflates while this thread parses the JPEGs
+        jpegs = [load(ds.real, image_key(R, i), "jpeg", R) for i in ids]
+        batch = I.DecodeBatch(jpegs + list(pngs))
         lbl = np.stack([(ds.flame_params[i] - ds.flame_mean) / ds.flame_std for i in ids]).astype(np.float32)
         pin = (lambda t: t.pin_memory()) if self.pin else (lambda t: t)
         # the renderer takes the raw rows: (p - m) / s * s + m is not p in float32
         raw = pin(torch.from_numpy(np.ascontiguousarray(ds.flame_params[ids], dtype=np.float32))) if render else None
-        return arena, offs, jb, pb, pin(torch.from_numpy(lbl)), pin(torch.tensor(ids, dtype=torch.int64)), raw, keys, rkeys
+        return batch, pin(torch.from_numpy(lbl)), pin(torch.tensor(ids, dtype=torch.int64)), raw
 
     def _launch(self, hb):
         """Enqueue the copy and the decode of one host batch on the side stream."""
         from . import image_decode as I
-        arena, offs, jb, pb, lbl, idx, raw, keys, rkeys = hb
+        batch, lbl, idx, raw = hb
         dev, B, R, rr = self.device, self.bs, self.ds.resolution, self.ds.rend_flm_res
         with torch.cuda.stream(self._stream):
-            d = arena.to(dev, non_blocking=True)
-            seg = lambda i: d[int(offs[i]):int(offs[i + 1])]
-            status = torch.zeros(3 * B, dtype=torch.int32, device=dev)
-            real_u8 = torch.empty(B, R, R, 3, dtype=torch.uint8, device=dev)
-            rend_u8 = torch.empty(2 * B, rr, rr, 3, dtype=torch.uint8, device=dev)
-            ws = torch.empty(jb.workspace_bytes, dtype=torch.uint8, device=dev)
-            jb.launch(seg(0), seg(2), real_u8, status[:B], ws)
+            images, status = batch.decode(dev)
+            real_u8 = I.as_batch(images[:B])
             if raw is None:
-                pb.launch(seg(1), seg(3), rend_u8, status[B:])
+                rend_u8 = I.as_batch(images[B:])
             else:
+                rend_u8 = torch.empty(2 * B, rr, rr, 3, dtype=torch.uint8, device=dev)
                 self.conditions.render_u8(raw.to(dev, non_blocking=True), out=rend_u8)
             if rr != R:
                 rend_u8 = I.resize_bicubic_u8(rend_u8, R)
@@ -505,16 +480,13 @@ class DeviceBatchLoader:
             st = status.to("cpu", non_blocking=True) if self.pin else status.cpu()
             done = torch.cuda.Event()
             done.record()
-        return (real, cond, labels, indices), st, done, keys + rkeys
+        return (real, cond, labels, indices), st, done, batch.names
 
     def _finish(self, launched):
         from . import image_decode as I
-        out, st, done, keys = launched
+        out, st, done, names = launched
         done.synchronize()                          # the side stream only: this batch's copy and decode
-        bad = np.flatnonzero(st.numpy())
-        if bad.size:
-            raise I.UnsupportedImage(f"{keys[bad[0]].decode()}: corrupt or truncated image data "
-                                     f"(device status {int(st[bad[0]])})")
+        I.check_status(st, names)
         cur = torch.cuda.current_stream(self.device)
         cur.wait_event(done)
         for t in out:                               # allocated on the side stream, used on this one
@@ -540,7 +512,7 @@ class DeviceBatchLoader:
                         return
                     ids = [int(self.ds.valid_ids[int(j)]) for j in order[b * self.bs:(b + 1) * self.bs]]
                     try:
-                        item = self._host_batch(ids, pool)
+                        item = self.host_batch(ids, pool)
                     except Exception as e:          # handed to the consumer, which raises it
                         item = e
                     ready.put(item)

@@ -9,8 +9,8 @@
   4. the FID Inception features (its own bilinear resize to 299 and 2x - 1), then ``np.mean`` / ``np.cov`` in float64.
 
 Here a host thread pool reads, parses and inflates the PNGs of batch k+1 (zlib releases the GIL) while the device undoes
-the scanline filters (``gifb200_png_unfilter``), resizes (``gifb200_resize_bicubic_u8``, bit-exact with Pillow) and runs the
-network on batch k.  The native ``InceptionV3`` takes the uint8 batch as it is (``gifb200_resize_bilinear_u8`` reads
+the scanline filters (``image_decode.DecodeBatch``), resizes (``gifb200_resize_bicubic_u8``, bit-exact with Pillow) and
+runs the network on batch k.  The native ``InceptionV3`` takes the uint8 batch as it is (``gifb200_resize_bilinear_u8`` reads
 v / 255 inside its input resize); any other model gets the float batch v / 255.  ``fid.ActivationStatistics`` reduces the
 features as they come.
 
@@ -48,58 +48,39 @@ def real_image_files(root, limit=MAX_IMAGES, batch_size=BATCH_SIZE):
 
 
 def load_png(path):
-    """Read, parse and inflate one PNG on the host: ((W, H, 3, b""), inflated scanlines).  8-bit RGB only."""
+    """Read, parse and inflate one PNG on the host (``image_decode.host_decode``): ((W, H, 3, b""), inflated scanlines).
+    8-bit RGB only."""
     with open(path, "rb") as f:
-        data = f.read()
-    try:
-        w, h, bpp, z = I.parse_png(data)
-        if bpp != 3:
-            raise I.UnsupportedImage(f"{'grey' if bpp == 1 else 'RGBA'} PNG: the FID statistics take 8-bit RGB images only")
-        return (w, h, bpp, b""), I.inflate_png((w, h, bpp, z))
-    except I.UnsupportedImage as e:
-        raise I.UnsupportedImage(f"{path}: {e}") from None
+        im = I.host_decode(f.read(), path)
+    if im.kind != "png" or im.bpp != 3:
+        what = "JPEG" if im.kind == "jpeg" else ("grey" if im.bpp == 1 else "RGBA") + " PNG"
+        raise I.UnsupportedImage(f"{path}: {what}: the FID statistics take 8-bit RGB PNGs only")
+    return (im.w, im.h, im.bpp, b""), im.data
 
 
-def _stage(files, loaded, resolution, device):
-    """Pack one batch into a pinned buffer (scanlines, then the descriptors) and copy it to the device without blocking."""
-    hdrs, raws = zip(*loaded)
+def device_batch(files, loaded, resolution, status, device):
+    """One batch of ``load_png`` results on the device (``image_decode.DecodeBatch``) as the network's input: uint8
+    (B, h, w, 3), the scanlines unfiltered and, where the reference resizes (R != 299 and the image is not already R x R),
+    Pillow's bicubic resize to R x R; a batch of one shape that needs no resize is returned as a view.  ``status``: int32
+    (B,) device words, zeroed by the caller, that receive the decode's status (``image_decode.check_status``)."""
+    hdrs = [h for h, _ in loaded]
     if resolution == INCEPTION_SIZE:
         for f, (w, h, _, _) in zip(files, hdrs):
             if (w, h) != hdrs[0][:2]:
                 raise ValueError(f"{f}: {w}x{h} in a batch of {hdrs[0][0]}x{hdrs[0][1]} images; at resolution 299 the images "
                                  "are not resized, so they must all have one size (the reference's np.array of the batch)")
-    pb = I.PngBatch(hdrs, raws)
-    off = -(-pb.data_bytes // 16) * 16
-    host = torch.empty(off + pb.desc.nbytes, dtype=torch.uint8, pin_memory=True)
-    a = host.numpy()
-    o = 0
-    for r in raws:
-        a[o:o + len(r)] = np.frombuffer(r, np.uint8)
-        o += len(r)
-    a[off:] = pb.desc.view(np.uint8).ravel()
-    dev = host.to(device, non_blocking=True)      # the host allocator keeps `host` until this copy has run
-    return pb, dev[:max(pb.data_bytes, 1)], dev[off:].view(torch.int32)
+    batch = I.DecodeBatch([I.HostImage(f, "png", w, h, bpp, raw) for f, ((w, h, bpp, _), raw) in zip(files, loaded)])
+    groups = I.shape_groups(batch.decode(device, status)[0])
 
-
-def device_batch(files, loaded, resolution, status, device):
-    """One batch of ``load_png`` results on the device as the network's input: uint8 (B, h, w, 3), the scanlines unfiltered
-    and, where the reference resizes (R != 299 and the image is not already R x R), Pillow's bicubic resize to R x R.
-    ``status``: int32 (B,) device words, nonzero for an image with corrupt scanlines (zeroed by the caller)."""
-    pb, data, desc = _stage(files, loaded, resolution, device)
-    out = torch.empty(pb.out_bytes, dtype=torch.uint8, device=device)
-    pb.launch(data, desc, out, status)
-    views = [out[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(pb.out_offsets, pb.shapes)]
-    shapes = sorted(set(pb.shapes))
-    if resolution == INCEPTION_SIZE or shapes == [(resolution, resolution)]:
-        return out.view(pb.n_img, *views[0].shape)
-    if len(shapes) == 1:
-        return I.resize_bicubic_u8(out.view(pb.n_img, *views[0].shape), resolution)
-    x = torch.empty(pb.n_img, resolution, resolution, 3, dtype=torch.uint8, device=device)
-    for shp in shapes:
-        idx = [i for i, s in enumerate(pb.shapes) if s == shp]
-        src = torch.stack([views[i] for i in idx])
-        x[idx] = src if shp == (resolution, resolution) else I.resize_bicubic_u8(src, resolution)
-    return x
+    def fit(x):
+        keep = resolution == INCEPTION_SIZE or x.shape[1:3] == (resolution, resolution)
+        return x if keep else I.resize_bicubic_u8(x, resolution)
+    if len(groups) == 1:
+        return fit(groups[0][1])
+    out = torch.empty(len(files), resolution, resolution, 3, dtype=torch.uint8, device=device)
+    for idx, x in groups:
+        out[idx] = fit(x)
+    return out
 
 
 def real_image_statistics(root, resolution, model, dims, batch_size=BATCH_SIZE, threads=None, device=None,
@@ -119,15 +100,11 @@ def real_image_statistics(root, resolution, model, dims, batch_size=BATCH_SIZE, 
     inflight = collections.deque()                 # at most two batches queued on the device ahead of the host
     pool = ThreadPoolExecutor(threads or min(32, os.cpu_count() or 1))
     try:
-        nxt = [pool.submit(load_png, f) for f in batches[0]]
         with torch.no_grad():
-            for k, names in enumerate(batches):
-                loaded = [p.result() for p in nxt]
-                if k + 1 < len(batches):
-                    nxt = [pool.submit(load_png, f) for f in batches[k + 1]]
+            for k, loaded in enumerate(I.prefetch(pool, load_png, batches)):
                 if len(inflight) == 2:
                     inflight.popleft().synchronize()
-                x = device_batch(names, loaded, resolution, status[k * bs:(k + 1) * bs], device)
+                x = device_batch(batches[k], loaded, resolution, status[k * bs:(k + 1) * bs], device)
                 if not native:                     # v / 255 with a true division (a CUDA 0-dim divisor, not a scalar)
                     x = x.permute(0, 3, 1, 2).float().div_(torch.full((), 255.0, device=device))
                 stats.update(compute_activation_batch(model, x))
@@ -136,10 +113,7 @@ def real_image_statistics(root, resolution, model, dims, batch_size=BATCH_SIZE, 
                 inflight.append(ev)
     finally:
         pool.shutdown(wait=True, cancel_futures=True)
-    bad = torch.nonzero(status).flatten().tolist()
-    if bad:
-        raise I.UnsupportedImage(f"{files[bad[0]]}: corrupt PNG scanlines (unknown filter type)"
-                                 + (f", and {len(bad) - 1} more files" if len(bad) > 1 else ""))
+    I.check_status(status.cpu(), files)
     return stats.finalize()
 
 

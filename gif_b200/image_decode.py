@@ -2,8 +2,10 @@
 
 The host does only what is cheap or inherently serial: it parses JPEG markers and PNG chunks, builds the Huffman and
 quantisation tables, removes JPEG byte stuffing and splits the scan at restart markers, checks PNG CRCs and inflates the
-IDAT stream with zlib (which releases the GIL).  ``JpegBatch`` / ``PngBatch`` pack what one batch needs into byte arenas, so a batch
-costs one host-to-device copy; ``decode_*`` then run the kernels of csrc/image_decode.cu on it:
+IDAT stream with zlib (which releases the GIL).  ``host_decode`` does this for one image and names it in every error it
+raises.  ``DecodeBatch`` packs a batch of such images, JPEG and PNG in any mix, into one pinned arena (``JpegBatch`` /
+``PngBatch`` lay out each kind), so a batch costs one host-to-device copy, and runs the kernels of csrc/image_decode.cu
+on it; ``check_status`` turns their per-image status words into an ``UnsupportedImage`` naming the image:
 
     JPEG  parallel entropy decode -> dequantise + islow IDCT -> fancy upsampling + YCbCr->RGB       (libjpeg-turbo defaults)
     PNG   scanline unfiltering (None/Sub/Up/Average/Paeth) -> RGB (grey replicated, alpha dropped)  (``convert("RGB")``)
@@ -17,6 +19,7 @@ import re
 import struct
 import zlib
 from functools import lru_cache
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -300,24 +303,6 @@ class JpegBatch:
                                                 workspace.numel(), _lib.stream()), "jpeg_decode")
 
 
-def _to_device(arr, device):
-    t = torch.from_numpy(np.frombuffer(arr, np.uint8).copy() if isinstance(arr, bytes) else np.ascontiguousarray(arr))
-    return t.to(device)
-
-
-def decode_jpeg_batch(blobs, device=None, chunk_bytes=CHUNK_BYTES):
-    """Decode baseline JPEG byte strings on the device.  Returns (images, status): a list of uint8 (H, W, 3) CUDA tensors
-    equal to ``np.asarray(Image.open(b).convert("RGB"))``, and int32 (n,) status words (0 = decoded; otherwise
-    STATUS_BAD_CODE / STATUS_BLOCK_COUNT bits: the entropy-coded data is corrupt or truncated)."""
-    device = torch.device(device or "cuda")
-    jb = JpegBatch([parse_jpeg(b) for b in blobs], chunk_bytes)
-    out = torch.empty(jb.out_bytes, dtype=torch.uint8, device=device)
-    status = torch.zeros(jb.n_img, dtype=torch.int32, device=device)
-    ws = torch.empty(jb.workspace_bytes, dtype=torch.uint8, device=device)
-    jb.launch(_to_device(jb.data + b"\0", device), _to_device(jb.ints, device), out, status, ws)
-    return [out[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(jb.out_offsets, jb.shapes)], status
-
-
 # ------------------------------------------------------------------------------------------------------------------- PNG
 _PNG_SIG = b"\x89PNG\r\n\x1a\n"
 _PNG_BPP = {0: 1, 2: 3, 6: 4}
@@ -404,17 +389,127 @@ class PngBatch:
                                                  out.data_ptr(), status.data_ptr(), _lib.stream()), "png_unfilter")
 
 
-def decode_png_batch(blobs, device=None):
-    """Decode 8-bit grey / RGB / RGBA PNG byte strings; the scanline filters are undone on the device.  Returns (images,
-    status) like ``decode_jpeg_batch``, images equal to ``np.asarray(Image.open(b).convert("RGB"))``."""
-    device = torch.device(device or "cuda")
-    hdrs = [parse_png(b) for b in blobs]
-    raws = [inflate_png(h) for h in hdrs]
-    pb = PngBatch(hdrs, raws)
-    out = torch.empty(pb.out_bytes, dtype=torch.uint8, device=device)
-    status = torch.zeros(pb.n_img, dtype=torch.int32, device=device)
-    pb.launch(_to_device(b"".join(raws), device), _to_device(pb.desc, device), out, status)
-    return [out[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(pb.out_offsets, pb.shapes)], status
+# --------------------------------------------------------------------------------------------------------------- batches
+class HostImage(NamedTuple):
+    """One image after ``host_decode``: its name (a path or a key), "jpeg" or "png", its size, bytes per pixel (JPEG
+    components, PNG channels) and what the device needs: ``parse_jpeg``'s result, or the inflated PNG scanlines."""
+    name: str
+    kind: str
+    w: int
+    h: int
+    bpp: int
+    data: object
+
+
+def host_decode(data, name):
+    """The host half of decoding one encoded image, dispatched on its magic bytes as ``Image.open`` does: a baseline JPEG
+    is parsed, a PNG parsed and inflated.  Every ``UnsupportedImage`` it raises starts with ``name``."""
+    try:
+        if data[:8] == _PNG_SIG:
+            hdr = parse_png(data)
+            return HostImage(name, "png", *hdr[:3], inflate_png(hdr))
+        if data[:3] == b"\xff\xd8\xff":
+            p = parse_jpeg(data)
+            return HostImage(name, "jpeg", p["w"], p["h"], p["ncomp"], p)
+        raise UnsupportedImage("not a PNG or baseline JPEG file (the device decoders read only these)")
+    except UnsupportedImage as e:
+        raise UnsupportedImage(f"{name}: {e}") from None
+
+
+class DecodeBatch:
+    """``host_decode`` results, JPEG and PNG in any mix, packed for one decode: the JPEG data, the JPEG int tables, the PNG
+    scanlines and the PNG descriptors in one host arena, 256-byte aligned sections, pinned when CUDA is available.  The
+    output buffer and the status words hold the JPEGs, then the PNGs, each kind in input order: ``order`` lists the input
+    indices and ``names`` the images' names in that order."""
+
+    def __init__(self, images, chunk_bytes=CHUNK_BYTES):
+        self.order = sorted(range(len(images)), key=lambda i: images[i].kind == "png")      # stable: JPEGs, then PNGs
+        self.names = [images[i].name for i in self.order]
+        jpegs, pngs = [im for im in images if im.kind == "jpeg"], [im for im in images if im.kind == "png"]
+        jb = self.jpeg = JpegBatch([im.data for im in jpegs], chunk_bytes) if jpegs else None
+        pb = self.png = PngBatch([(im.w, im.h, im.bpp, b"") for im in pngs], [im.data for im in pngs]) if pngs else None
+        starts = np.cumsum([0] + [im.w * im.h * 3 for im in jpegs + pngs])            # the images back to back
+        self.out_bytes, self.png_out = int(starts[-1]), int(starts[len(jpegs)])
+        self.views = [None] * len(images)                                              # input order
+        for k, i in enumerate(self.order):
+            self.views[i] = (int(starts[k]), images[i].h, images[i].w)
+        sections = [[jb.data] if jb else [], [im.data for im in pngs], [jb.ints] if jb else [], [pb.desc] if pb else []]
+        sections = [[np.frombuffer(b, np.uint8) for b in s] for s in sections]
+        self.offsets = np.cumsum([0] + [-(-sum(b.size for b in s) // 256) * 256 for s in sections])
+        self.arena = torch.empty(int(self.offsets[-1]), dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+        a = self.arena.numpy()
+        for o, s in zip(self.offsets, sections):
+            for b in s:
+                a[o:o + b.size] = b
+                o += b.size
+
+    def decode(self, device, status=None):
+        """Enqueue one non-blocking copy of the arena and the decode kernels on the current stream.  Returns (images,
+        status): uint8 (H, W, 3) device views in input order, equal to ``np.asarray(Image.open(b).convert("RGB"))``, and
+        int32 device status words in ``order`` (0 = decoded; otherwise STATUS_* bits: corrupt or truncated data), written
+        to ``status`` (zeroed, one word per image) when the caller passes one."""
+        d = self.arena.to(device, non_blocking=True)      # the host allocator keeps the arena until this copy has run
+        sec = [d[int(lo):int(hi)] for lo, hi in zip(self.offsets[:-1], self.offsets[1:])]
+        out = torch.empty(self.out_bytes, dtype=torch.uint8, device=device)
+        status = torch.zeros(len(self.order), dtype=torch.int32, device=device) if status is None else status
+        if self.jpeg:
+            ws = torch.empty(self.jpeg.workspace_bytes, dtype=torch.uint8, device=device)
+            self.jpeg.launch(sec[0], sec[2], out, status, ws)
+        if self.png:
+            self.png.launch(sec[1], sec[3], out[self.png_out:], status[len(self.order) - self.png.n_img:])
+        return [out[o:o + h * w * 3].view(h, w, 3) for o, h, w in self.views], status
+
+
+def check_status(status, names):
+    """Raise ``UnsupportedImage`` naming the first image whose status word is nonzero and counting the others.
+    ``status``: host-side words, one per name."""
+    st = np.asarray(status)
+    bad = np.flatnonzero(st)
+    if bad.size:
+        s = int(st[bad[0]])
+        what = "corrupt PNG scanlines (unknown filter type)" if s & STATUS_PNG_FILTER else "corrupt or truncated JPEG data"
+        raise UnsupportedImage(f"{names[bad[0]]}: {what} (device status {s})"
+                               + (f", and {bad.size - 1} more images" if bad.size > 1 else ""))
+
+
+def decode_images(blobs, device=None, chunk_bytes=CHUNK_BYTES):
+    """Decode encoded images (baseline JPEG; 8-bit grey, RGB or RGBA PNG) on the device, through ``DecodeBatch``.  Returns
+    (images, status) as ``DecodeBatch.decode`` does, but with the status words in input order."""
+    batch = DecodeBatch([host_decode(b, f"image {i}") for i, b in enumerate(blobs)], chunk_bytes)
+    images, status = batch.decode(torch.device(device or "cuda"))
+    return images, status[torch.as_tensor(np.argsort(batch.order), device=status.device)]
+
+
+decode_jpeg_batch = decode_png_batch = decode_images       # the names of the former per-format decoders
+
+
+def as_batch(images):
+    """Same-shape uint8 (H, W, 3) images -> (n, H, W, 3): a view when they lie back to back in one buffer (a run of one
+    kind in ``DecodeBatch.decode``'s output), else a stacked copy."""
+    x = images[0]
+    step = x.numel()
+    if all(y.shape == x.shape and y.is_contiguous() and y.untyped_storage().data_ptr() == x.untyped_storage().data_ptr()
+           and y.data_ptr() == x.data_ptr() + k * step for k, y in enumerate(images)):
+        return x.as_strided((len(images),) + tuple(x.shape), (step,) + x.stride())
+    return torch.stack(images)
+
+
+def shape_groups(images):
+    """Images of one batch grouped by shape, in sorted shape order: [(input indices, uint8 (n, H, W, 3) ``as_batch``)]."""
+    groups = {}
+    for i, x in enumerate(images):
+        groups.setdefault(tuple(x.shape), []).append(i)
+    return [(idx, as_batch([images[i] for i in idx])) for _, idx in sorted(groups.items())]
+
+
+def prefetch(pool, load, batches):
+    """Yield ``[load(x) for x in batch]`` for each batch in turn.  The loads run on ``pool``; the next batch's are submitted
+    when this one is taken, so they run while the caller works on this one."""
+    futures = [pool.submit(load, x) for x in batches[0]] if batches else []
+    for nxt in list(batches[1:]) + [[]]:
+        done = [f.result() for f in futures]
+        futures = [pool.submit(load, x) for x in nxt]
+        yield done
 
 
 # ---------------------------------------------------------------------------------------------------------------- resize

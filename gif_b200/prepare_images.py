@@ -23,7 +23,6 @@ import threading
 import zlib
 from concurrent.futures import ThreadPoolExecutor
 
-import numpy as np
 import torch
 
 from . import image_decode as I
@@ -93,80 +92,32 @@ def _jpeg_comment(data):
 
 
 def load_image(path):
-    """Read and host-decode one file, dispatched on its magic bytes as ``Image.open`` does: ("png", (header, inflated
-    scanlines)) or ("jpeg", parsed markers), and its comment.  Anything else raises ``UnsupportedImage`` naming the file."""
+    """Read and host-decode one file (``image_decode.host_decode``: dispatched on its magic bytes as ``Image.open`` does):
+    (the ``HostImage``, its comment).  Anything the device decoders cannot read raises ``UnsupportedImage`` naming the file."""
     with open(path, "rb") as f:
         data = f.read()
-    try:
-        if data[:8] == I._PNG_SIG:
-            hdr = I.parse_png(data)
-            return "png", (hdr[:3] + (b"",), I.inflate_png(hdr)), _png_comment(data)
-        if data[:3] == b"\xff\xd8\xff":
-            return "jpeg", I.parse_jpeg(data), _jpeg_comment(data)
-        raise I.UnsupportedImage("not a PNG or baseline JPEG file (the device decoders read only these)")
-    except I.UnsupportedImage as e:
-        raise I.UnsupportedImage(f"{path}: {e}") from None
+    im = I.host_decode(data, path)
+    return im, (_png_comment if im.kind == "png" else _jpeg_comment)(data)
 
 
-def _upload(parts, device):
-    """Byte strings -> one uint8 device tensor, staged in pinned memory so the copy runs at full speed without blocking (the
-    host allocator keeps the staging buffer until the copy has run)."""
-    host = torch.empty(max(1, sum(len(p) for p in parts)), dtype=torch.uint8, pin_memory=True)
-    a, o = host.numpy(), 0
-    for p in parts:
-        a[o:o + len(p)] = np.frombuffer(p, np.uint8)
-        o += len(p)
-    return host.to(device, non_blocking=True)
-
-
-def _decode(files, loaded, device):
-    """One batch of ``load_image`` results -> list of uint8 (H, W, 3) device tensors (Image.convert("RGB"))."""
-    out = [None] * len(files)
-    for kind in ("png", "jpeg"):
-        idx = [i for i, l in enumerate(loaded) if l[0] == kind]
-        if not idx:
-            continue
-        if kind == "png":
-            hdrs, raws = zip(*(loaded[i][1] for i in idx))
-            pb = I.PngBatch(hdrs, raws)
-            buf = torch.empty(pb.out_bytes, dtype=torch.uint8, device=device)
-            status = torch.zeros(pb.n_img, dtype=torch.int32, device=device)
-            pb.launch(_upload(raws, device), I._to_device(pb.desc, device), buf, status)
-            shapes, offs = pb.shapes, pb.out_offsets
-        else:
-            jb = I.JpegBatch([loaded[i][1] for i in idx])
-            buf = torch.empty(jb.out_bytes, dtype=torch.uint8, device=device)
-            status = torch.zeros(jb.n_img, dtype=torch.int32, device=device)
-            ws = torch.empty(jb.workspace_bytes, dtype=torch.uint8, device=device)
-            jb.launch(_upload([jb.data, b"\0"], device), I._to_device(jb.ints, device), buf, status, ws)
-            shapes, offs = jb.shapes, jb.out_offsets
-        bad = torch.nonzero(status).flatten().tolist()
-        if bad:
-            raise I.UnsupportedImage(f"{files[idx[bad[0]]]}: corrupt {kind.upper()} data")
-        for k, i in enumerate(idx):
-            h, w = shapes[k]
-            out[i] = buf[offs[k]:offs[k] + h * w * 3].view(h, w, 3)
-    return out
-
-
-def shape_groups(images):
-    """Images of one batch grouped by shape: [(indices, uint8 (n, H, W, 3))], so each group is resized in one call."""
-    shapes = sorted({tuple(x.shape[:2]) for x in images})
-    groups = []
-    for shp in shapes:
-        idx = [i for i, x in enumerate(images) if tuple(x.shape[:2]) == shp]
-        groups.append((idx, torch.stack([images[i] for i in idx])))
-    return groups
+def decoded_groups(loaded, device):
+    """One batch of ``load_image`` results decoded on the device (Image.convert("RGB")) and grouped by shape
+    (``image_decode.shape_groups``), so each group is resized in one call.  A corrupt image raises ``UnsupportedImage``
+    naming its file."""
+    batch = I.DecodeBatch([im for im, _ in loaded])
+    images, status = batch.decode(device)
+    I.check_status(status.cpu(), batch.names)
+    return I.shape_groups(images)
 
 
 def resized_crops(groups, n, size):
-    """``shape_groups`` of n images -> (n, size, size, 3): torchvision's resize(size, LANCZOS) + center_crop(size) of each,
-    Pillow-exact."""
+    """``decoded_groups`` of n images -> (n, size, size, 3): torchvision's resize(size, LANCZOS) + center_crop(size) of
+    each, Pillow-exact."""
     out = None
     for idx, x in groups:
         (rw, rh), (left, top) = I.resized_crop_box(x.shape[2], x.shape[1], size)
         r = I.resize_lanczos_u8(x, (rh, rw))[:, top:top + size, left:left + size]
-        if len(groups) == 1:
+        if idx == list(range(n)):                  # one group, the whole batch in input order
             return r.contiguous()
         if out is None:
             out = torch.empty(n, size, size, 3, dtype=torch.uint8, device=x.device)
@@ -208,16 +159,12 @@ def prepare_multiscale_lmdb(root, out, sizes=SIZES, quality=100, batch_size=32, 
             th = threading.Thread(target=write, args=(w,), daemon=True)
             th.start()
             try:
-                nxt = [pool.submit(load_image, f) for f in batches[0]]
-                for k, names in enumerate(batches):
-                    loaded = [p.result() for p in nxt]
-                    if k + 1 < len(batches):
-                        nxt = [pool.submit(load_image, f) for f in batches[k + 1]]
-                    groups = shape_groups(_decode(names, loaded, device))
-                    comments = [l[2] for l in loaded]
+                for k, loaded in enumerate(I.prefetch(pool, load_image, batches)):
+                    groups = decoded_groups(loaded, device)
+                    comments = [c for _, c in loaded]
                     first = k * batch_size
                     for s in sizes:
-                        blobs = encode_jpeg_batch(resized_crops(groups, len(names), s), quality, comments)
+                        blobs = encode_jpeg_batch(resized_crops(groups, len(loaded), s), quality, comments)
                         values.put([(image_key(s, first + i), b) for i, b in enumerate(blobs)])
                     if writer_error:
                         break

@@ -1,10 +1,12 @@
 """CPU: the host side of the device image decoders -- JPEG marker and PNG chunk parsing on Pillow-written files, the
-rejection of everything outside the supported subset, and Pillow's bicubic coefficient tables."""
+rejection of everything outside the supported subset, Pillow's bicubic coefficient tables, and the shared batch path
+(``host_decode``, ``DecodeBatch``'s packing, ``check_status``, shape grouping, ``prefetch``)."""
 import struct
 import zlib
 
 import numpy as np
 import pytest
+import torch
 from PIL import Image
 
 from gif_b200 import image_decode as I
@@ -137,3 +139,78 @@ def test_bicubic_coeffs(sizes):
         dense[r, c[r, 0]:c[r, 0] + c[r, 1]] = c[r, 2:2 + c[r, 1]]
     mine = np.clip(((255 * dense + (1 << 21)) >> 22), 0, 255)
     assert np.array_equal(mine, pillow_coeffs(i, o))
+
+
+# ---------------------------------------------------------------------------------------------------------------- batches
+def test_host_decode_dispatches_and_names_the_image():
+    p = I.host_decode(png(photo(5, 7, 1, "RGBA")), "a.png")
+    assert (p.name, p.kind, p.w, p.h, p.bpp, len(p.data)) == ("a.png", "png", 7, 5, 4, 5 * (1 + 7 * 4))
+    j = I.host_decode(jpeg(photo(9, 11, 2)), "k-00001")
+    assert (j.kind, j.w, j.h, j.bpp) == ("jpeg", 11, 9, 3) and j.data["segments"]
+    bad = bytearray(png(photo(16, 16, 5)))
+    bad[40] ^= 0x55
+    for blob, msg in ((b"GIF89a" + bytes(20), "not a PNG or baseline JPEG"), (bytes(bad), "CRC"),
+                      (jpeg(photo(32, 32, 3), progressive=True), "progressive")):
+        with pytest.raises(I.UnsupportedImage, match=f"^img/x.bin: .*{msg}"):
+            I.host_decode(blob, "img/x.bin")
+
+
+def test_decode_batch_packs_a_mixed_batch_in_one_arena():
+    imgs = [I.host_decode(png(photo(5, 7, 1)), "p0"), I.host_decode(jpeg(photo(9, 11, 2)), "j0"),
+            I.host_decode(png(photo(3, 4, 3, "L")), "p1"), I.host_decode(jpeg(photo(17, 33, 4), quality=100), "j1")]
+    b = I.DecodeBatch(imgs)
+    assert b.order == [1, 3, 0, 2] and b.names == ["j0", "j1", "p0", "p1"]
+    jb, pb = b.jpeg, b.png
+    assert (jb.n_img, pb.n_img) == (2, 2) and b.out_bytes == jb.out_bytes + pb.out_bytes == b.png_out + pb.out_bytes
+    # views in input order: the JPEGs at their JpegBatch offsets, then the PNGs after them
+    assert b.views == [(jb.out_bytes + pb.out_offsets[0], 5, 7), (jb.out_offsets[0], 9, 11),
+                       (jb.out_bytes + pb.out_offsets[1], 3, 4), (jb.out_offsets[1], 17, 33)]
+    a, o = b.arena.numpy(), b.offsets
+    assert (np.diff(o) % 256 == 0).all() and len(o) == 5
+    assert a[o[0]:o[0] + len(jb.data)].tobytes() == jb.data
+    assert a[o[1]:o[1] + pb.data_bytes].tobytes() == imgs[0].data + imgs[2].data
+    assert np.array_equal(a[o[2]:o[2] + jb.ints.nbytes].view(np.int32), jb.ints)
+    assert np.array_equal(a[o[3]:o[3] + pb.desc.nbytes].view(np.int32), pb.desc.ravel())
+    only_png = I.DecodeBatch(imgs[::2])
+    assert only_png.jpeg is None and only_png.order == [0, 1] and only_png.png_out == 0
+
+
+def test_check_status_names_the_first_bad_image():
+    I.check_status(np.zeros(3, np.int32), ["a", "b", "c"])
+    with pytest.raises(I.UnsupportedImage, match=r"^b: corrupt or truncated JPEG data \(device status 1\), and 1 more images$"):
+        I.check_status(np.array([0, I.STATUS_BAD_CODE, 0, I.STATUS_PNG_FILTER]), ["a", "b", "c", "d"])
+    with pytest.raises(I.UnsupportedImage, match=r"^c: corrupt PNG scanlines .*status 4\)$"):
+        I.check_status(torch.tensor([0, 0, I.STATUS_PNG_FILTER], dtype=torch.int32), ["a", "b", "c"])
+
+
+def test_shape_groups_view_when_back_to_back():
+    """A group lying back to back in the output buffer is returned as a view of it; otherwise it is stacked in input
+    order.  A batch laid out by kind (JPEGs first) with one shape is one group with the identity indices."""
+    buf = torch.arange(4 * 2 * 3 * 3 + 2 * 5 * 5 * 3, dtype=torch.int64).to(torch.uint8)
+    a = [buf[k * 18:(k + 1) * 18].view(2, 3, 3) for k in range(4)]
+    b = [buf[72 + k * 75:72 + (k + 1) * 75].view(5, 5, 3) for k in range(2)]
+    groups = I.shape_groups([a[0], b[0], a[1], a[2], b[1], a[3]])
+    assert [idx for idx, _ in groups] == [[0, 2, 3, 5], [1, 4]]
+    for (idx, x), src in zip(groups, (a, b)):
+        assert x.data_ptr() == src[0].data_ptr() and torch.equal(x, torch.stack(src))       # views
+    mixed = [a[2], a[0], a[3], a[1]]                                                         # input order != buffer order
+    (idx, x), = I.shape_groups(mixed)
+    assert idx == [0, 1, 2, 3] and torch.equal(x, torch.stack(mixed)) and x.data_ptr() != a[0].data_ptr()
+    assert torch.equal(I.as_batch([a[0], a[2]]), torch.stack([a[0], a[2]]))                   # a gap: a copy
+
+
+def test_prefetch_runs_the_next_batch_while_this_one_is_used():
+    from concurrent.futures import ThreadPoolExecutor
+    batches = [[1, 2], [3], [4, 5, 6]]
+    submitted = []
+
+    class Pool(ThreadPoolExecutor):
+        def submit(self, fn, x):
+            submitted.append(x)
+            return super().submit(fn, x)
+    with Pool(2) as pool:
+        got = []
+        for k, r in enumerate(I.prefetch(pool, lambda x: 10 * x, batches)):
+            got.append(r)
+            assert submitted == sum(batches[:k + 2], [])           # batch k+1 is on the pool while batch k is used
+    assert got == [[10, 20], [30], [40, 50, 60]]

@@ -68,7 +68,7 @@ def render_leg(row, real, R, bs, reps, cr):
     loader = DeviceBatchLoader(ds, bs, conditions=cr)
     ids = list(range(bs))
     with ThreadPoolExecutor(loader.threads) as pool:
-        row["render_loader_host_cpu_s"] = cpu_per_batch(lambda: loader._host_batch(ids, pool), reps)
+        row["render_loader_host_cpu_s"] = cpu_per_batch(lambda: loader.host_batch(ids, pool), reps)
     raw = torch.from_numpy(params).cuda()
     out = torch.empty(2 * bs, 256, 256, 3, dtype=torch.uint8, device="cuda")
     row["render_ms"] = event_ms(lambda: cr.render_u8(raw, out=out))
@@ -79,7 +79,7 @@ def render_leg(row, real, R, bs, reps, cr):
 def decode_leg(R, bs, reps, chunks, cr=None):
     from concurrent.futures import ThreadPoolExecutor
     from gif_b200 import image_decode as I
-    from gif_b200.data import DeviceBatchLoader, GifLmdbDataset
+    from gif_b200.data import DeviceBatchLoader, GifLmdbDataset, image_key, normal_map_key
     from gif_b200.synth_images import build_lmdbs
     with tempfile.TemporaryDirectory() as tmp:
         real, rend = build_lmdbs(tmp, bs, R, 256)
@@ -88,29 +88,32 @@ def decode_leg(R, bs, reps, chunks, cr=None):
         pil = cpu_per_batch(lambda: [ds[i] for i in ids], reps)
         loader = DeviceBatchLoader(ds, bs)
         with ThreadPoolExecutor(loader.threads) as pool:
-            dev_host = cpu_per_batch(lambda: loader._host_batch(ids, pool), reps)
-            hb = loader._host_batch(ids, pool)
+            dev_host = cpu_per_batch(lambda: loader.host_batch(ids, pool), reps)
         row = {"resolution": R, "batch": bs, "pil_cpu_s": pil, "device_loader_host_cpu_s": dev_host,
                "host_cpu_ratio": pil / dev_host}
         if not torch.cuda.is_available():
             return row
-        arena, offs, jb, pb = hb[:4]
-        d = arena.cuda()
-        seg = lambda i: d[int(offs[i]):int(offs[i + 1])]
+        # each kernel on its own: the loader's records, packed and uploaded here
+        jpegs = [I.host_decode(ds.real.get(image_key(R, i)), str(i)) for i in ids]
+        pngs = [I.host_decode(ds.rend.get(key(256, i)), str(i)) for key in (image_key, normal_map_key) for i in ids]
+        to_dev = lambda b: torch.from_numpy(np.frombuffer(b, np.uint8).copy()).cuda()
+        jb = I.JpegBatch([im.data for im in jpegs])
+        data = to_dev(jb.data)
         out = torch.empty(jb.out_bytes, dtype=torch.uint8, device="cuda")
         st = torch.zeros(3 * bs, dtype=torch.int32, device="cuda")
-        parsed = [I.parse_jpeg(ds.real.get(k)) for k in hb[7]]
         ref = None
         for cb in chunks:
-            b = I.JpegBatch(parsed, cb)
+            b = I.JpegBatch([im.data for im in jpegs], cb)
             ints = torch.from_numpy(b.ints).cuda()
             ws = torch.empty(b.workspace_bytes, dtype=torch.uint8, device="cuda")
-            row[f"jpeg_ms_chunk{cb}"] = event_ms(lambda: b.launch(seg(0), ints, out, st[:bs], ws))
+            row[f"jpeg_ms_chunk{cb}"] = event_ms(lambda: b.launch(data, ints, out, st[:bs], ws))
             ref = out.clone() if ref is None else ref
             assert torch.equal(out, ref) and (st.cpu() == 0).all(), cb     # every chunk size decodes the same bits
+        pb = I.PngBatch([(im.w, im.h, im.bpp, b"") for im in pngs], [im.data for im in pngs])
+        scan, desc = to_dev(b"".join(im.data for im in pngs)), torch.from_numpy(pb.desc).cuda()
         rend_u8 = torch.empty(2 * bs, 256, 256, 3, dtype=torch.uint8, device="cuda")
-        work = seg(1).clone()
-        row["png_ms"] = event_ms(lambda: (work.copy_(seg(1)), pb.launch(work, seg(3), rend_u8, st[bs:])))
+        work = scan.clone()
+        row["png_ms"] = event_ms(lambda: (work.copy_(scan), pb.launch(work, desc, rend_u8, st[bs:])))
         if R != 256:
             row["resize_ms"] = event_ms(lambda: I.resize_bicubic_u8(rend_u8, R))
         row["jpeg_entropy_bytes"], row["png_inflated_bytes"] = len(jb.data), pb.data_bytes

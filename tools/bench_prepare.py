@@ -33,16 +33,16 @@ def reference_worker(args):
     return out
 
 
-def profile_batch(P, encode_jpeg_batch, names, loaded):
+def profile_batch(P, encode_jpeg_batch, loaded):
     """Device time (ms) per kernel / copy name over one batch: decode, then the resizes and encodes of every size."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     dev = torch.device("cuda")
     for _ in range(2):                                   # the first pass warms up
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            groups = P.shape_groups(P._decode(names, loaded, dev))
+            groups = P.decoded_groups(loaded, dev)
             for s in P.SIZES:
-                encode_jpeg_batch(P.resized_crops(groups, len(names), s))
+                encode_jpeg_batch(P.resized_crops(groups, len(loaded), s))
             torch.cuda.synchronize()
     rows = [(e.key, e.device_time_total / 1e3, e.count) for e in prof.key_averages() if e.device_time_total > 0]
     return {k: {"ms": round(t, 3), "calls": c} for k, t, c in sorted(rows, key=lambda r: -r[1])[:25]}
@@ -92,7 +92,7 @@ def main():
         t0 = time.perf_counter()
         for k in range(0, len(files), a.batch_size):
             names = files[k:k + a.batch_size]
-            groups = P.shape_groups(P._decode(names, loaded[k:k + a.batch_size], torch.device("cuda")))
+            groups = P.decoded_groups(loaded[k:k + a.batch_size], torch.device("cuda"))
             for s in P.SIZES:
                 blobs = encode_jpeg_batch(P.resized_crops(groups, len(names), s))
                 values += [(image_key(s, k + i), b) for i, b in enumerate(blobs)]
@@ -116,7 +116,7 @@ def main():
         mine = dict(values)
         res["equal_to_reference"] = all(mine[image_key(s, i)] == ref[i][j] for i in range(a.n) for j, s in enumerate(P.SIZES))
         if a.profile:
-            res["profile_ms_per_batch"] = profile_batch(P, encode_jpeg_batch, files[:a.batch_size], loaded[:a.batch_size])
+            res["profile_ms_per_batch"] = profile_batch(P, encode_jpeg_batch, loaded[:a.batch_size])
     res["card_after"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm", "--format=csv,noheader"],
                                        capture_output=True, text=True).stdout.strip()
     if a.out:
