@@ -111,7 +111,35 @@ def _round_tf32_raw(x):
     check(lib.gifb200_axpby(ptr(x), None, ptr(y), x.numel(), 1.0, 0.0, 1, stream()), "gifb200_axpby(round)")
     return y
 
-PROFILE = None   # bench.py sets this to a list; every tensor-core conv launch then appends (ev0, ev1, flops, tag)
+
+def _tc_operand(x, path, planes=None):
+    """What a convolution kernel on ``path`` reads for the fp32 operand x: 3 (bf16x3) its split planes (``planes`` when the
+    caller already has them); 2 (tf32) x when it is marked tf32-representable, else a rounded and marked copy (the tensor
+    cores truncate, see gifb200.h); any other path (exact fp32 SIMT) x itself."""
+    if path == 3:
+        return planes if planes is not None else _planes(x)
+    if path == 2 and not _is_tf32(x):
+        return _tag(_round_tf32_raw(x), True)
+    return x
+
+
+PROFILE = None   # bench.py sets this to a list; every tensor-core conv launch then appends (ev0, ev1, flops, tag, key)
+
+
+def _profiled(on, launch, tag, key, out_hw):
+    """Runs ``launch()``.  When PROFILE is a list and ``on``, the launch is bracketed by CUDA events and PROFILE receives
+    (ev0, ev1, algorithmic flops, tag, key), key = (kind, mode, B, Hi, Wi, Ci, Co, k)."""
+    if PROFILE is None or not on:
+        launch()
+        return
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record()
+    launch()
+    ev1.record()
+    _, mode, B, Hi, Wi, Ci, Co, k = key
+    pix = Hi * Wi if mode == T2 else out_hw[0] * out_hw[1]          # algorithmic MACs: taps * Ci * Co per site
+    PROFILE.append((ev0, ev1, 2.0 * B * pix * Ci * Co * k * k, tag, key))
+
 
 _ws_cache = {}
 _ws_retired = []
@@ -156,34 +184,24 @@ def _conv_raw(x, w, k, mode, flip, transposed, out_hw, epilogue=None, planes=Non
     Ho, Wo = out_hw
     y = torch.empty((B, Ho, Wo, Co), dtype=torch.float32, device=x.device)
     nws = lib.gifb200_conv2d_workspace_bytes(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, int(transposed), CONV_IMPL)
-    impl, xin = CONV_IMPL, x
-    if CONV_IMPL == 3:
-        if nws > 0:
-            xin = planes if planes is not None else _planes(x)   # compensated tensor-core path: the kernel reads the split planes
-        else:
-            impl = 1                         # shape outside the tensor-core path: exact fp32 SIMT
-    elif nws > 0 and not _is_tf32(x):        # tensor-core path: operands must be tf32-representable (see gifb200.h)
-        x = xin = _tag(_round_tf32_raw(x), True)
+    path = 1 if nws == 0 else (3 if CONV_IMPL == 3 else 2)
+    impl = 1 if CONV_IMPL == 3 and path == 1 else CONV_IMPL     # shape outside the tensor-core path: exact fp32 SIMT
+    xin = _tc_operand(x, path, planes)
+    if path == 2:
+        x = xin
     ws, staged = _staged_workspace(w, nws, flip, transposed, impl, (Ci, Co, k), x.device)
     if staged:
         impl |= 0x10                             # GIFB200_CONV_PRESTAGED: skip the staging pass
-    prof = PROFILE is not None and nws > 0
-    if prof:
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
     if epilogue is None:
         act, bias, slope, gain, rt = 0, None, 1.0, 1.0, 0
     else:
         bias, slope, gain, rt = epilogue
         act = 1
-    check(lib.gifb200_conv2d(ptr(xin), ptr(w), ptr(y), B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, int(flip), int(transposed),
-                             impl, act, ptr(bias), float(slope), float(gain), int(rt), ptr(ws), nws, stream()),
-          "gifb200_conv2d")
-    if prof:
-        ev1.record()
-        pix = Hi * Wi if mode == T2 else Ho * Wo                    # algorithmic MACs: taps * Ci * Co per site
-        tag = "northstar" if (mode == S1 and Ci == 128 and Co == 128 and Ho == 256 and k == 3) else ""
-        PROFILE.append((ev0, ev1, 2.0 * B * pix * Ci * Co * k * k, tag, ("conv", mode, B, Hi, Wi, Ci, Co, k)))
+    tag = "northstar" if (mode == S1 and Ci == 128 and Co == 128 and Ho == 256 and k == 3) else ""
+    _profiled(nws > 0, lambda: check(lib.gifb200_conv2d(ptr(xin), ptr(w), ptr(y), B, Hi, Wi, Ci, Ho, Wo, Co, k, mode,
+                                                        int(flip), int(transposed), impl, act, ptr(bias), float(slope),
+                                                        float(gain), int(rt), ptr(ws), nws, stream()), "gifb200_conv2d"),
+              tag, ("conv", mode, B, Hi, Wi, Ci, Co, k), out_hw)
     return y, x
 
 
@@ -195,28 +213,15 @@ def _wgrad_raw(x, gy, k, mode, flip, transposed, x_planes=None):
     gw = torch.empty(shape, dtype=torch.float32, device=x.device)
     impl = 1 if CONV_IMPL == 1 else (3 if CONV_IMPL == 3 else WGRAD_IMPL)
     path = lib.gifb200_conv2d_wgrad_path(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, impl)
-    xin, gin = x, gy
-    if path == 3:                              # compensated contraction on the split planes of both operands
-        xin, gin = (x_planes if x_planes is not None else _planes(x)), _planes(gy)
-    elif path == 2:                            # MN-major tf32 path: operands must be tf32-representable
-        if not _is_tf32(x):
-            xin = _round_tf32_raw(x)
-        if not _is_tf32(gy):
-            gin = _round_tf32_raw(gy)
-    elif impl == 3:
+    xin, gin = _tc_operand(x, path, x_planes), _tc_operand(gy, path)
+    if impl == 3 and path != 3:
         impl = 1                               # shape outside the tensor-core path: exact fp32 SIMT
     nws = lib.gifb200_conv2d_wgrad_workspace_bytes(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, impl)
     ws = _workspace(nws, x.device)
-    prof = PROFILE is not None
-    if prof:
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
-    check(lib.gifb200_conv2d_wgrad(ptr(xin), ptr(gin), ptr(gw), B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, int(flip),
-                                   int(transposed), impl, ptr(ws), nws, stream()), "gifb200_conv2d_wgrad")
-    if prof:
-        ev1.record()
-        pix = Hi * Wi if mode == T2 else Ho * Wo
-        PROFILE.append((ev0, ev1, 2.0 * B * pix * Ci * Co * k * k, "wgrad", ("wgrad", mode, B, Hi, Wi, Ci, Co, k)))
+    _profiled(True, lambda: check(lib.gifb200_conv2d_wgrad(ptr(xin), ptr(gin), ptr(gw), B, Hi, Wi, Ci, Ho, Wo, Co, k, mode,
+                                                          int(flip), int(transposed), impl, ptr(ws), nws, stream()),
+                                  "gifb200_conv2d_wgrad"),
+              "wgrad", ("wgrad", mode, B, Hi, Wi, Ci, Co, k), (Ho, Wo))
     return gw
 
 
@@ -232,25 +237,23 @@ def _x3_backward_on_planes(x_shape, gy_shape, k, mode):
     return lib.gifb200_conv2d_wgrad_path(B, Hi, Wi, Ci, Ho, Wo, Co, k, mode, 3) == 3
 
 
-def _planes_carrier(like, planes):
-    """A gradient whose values exist ONLY as bf16x3 planes: an unwritten fp32 tensor of the right shape carrying them.  Used
-    strictly between a fused backward kernel and the two tensor-core contractions that consume it (_x3_backward_on_planes)."""
-    t = torch.empty_like(like)
-    t._gifb200_planes = (t._version, planes)
-    return t
-
-
 class _Conv(torch.autograd.Function):
-    """y = conv(x; W) with W addressed in the physical buffer w[T][R][S] (see gifb200.h)."""
+    """y = conv(x; W) with W addressed in the physical buffer w[T][R][S] (see gifb200.h).  With ``act`` = (slope, gain, rt),
+    y = lrelu(conv(x; w) + bias, slope) * gain in ONE kernel (fused epilogue of gifb200_conv2d; ``bias`` may be None):
+    ConvLayer = EqualConv2d -> FusedLeakyReLU (cl.py:752-799), nn.Conv2d(+ReLU) of NoiseInjection (cl.py:405-414).  The
+    backward is composed of the differentiable primitives (activation backward from the saved OUTPUT, adjoint conv, wgrad)."""
 
     @staticmethod
-    def forward(ctx, x_arg, w, k, mode, flip, transposed, out_hw):
+    def forward(ctx, x_arg, w, bias, k, mode, flip, transposed, out_hw, act):
         x, w = _c(x_arg), _c(w)
-        y, x_used = _conv_raw(x, w, k, mode, flip, transposed, out_hw)
+        epilogue = None if act is None else (None if bias is None else _c(bias.reshape(-1)),) + act
+        y, x_used = _conv_raw(x, w, k, mode, flip, transposed, out_hw, epilogue)
         # the (possibly tf32-rounded) operand is what wgrad re-reads; a rounded copy is outside the autograd graph, so a
         # recorded (create_graph) backward takes the weight gradient of the input itself (_wgrad_raw rounds it again)
-        ctx.save_for_backward(x_used, w, x_arg if x_used is not x and ctx.needs_input_grad[0] else None)
-        ctx.cfg = (k, mode, flip, transposed, tuple(x.shape[1:3]), _is_tf32(x_used))
+        ctx.save_for_backward(x_used, w, x_arg if x_used is not x and ctx.needs_input_grad[0] else None,
+                              None if act is None else y)
+        ctx.cfg = (k, mode, flip, transposed, tuple(x.shape[1:3]), _is_tf32(x_used), act,
+                   None if bias is None else bias.shape)
         c = getattr(x_used, "_gifb200_planes", None)
         ctx.planes = c[1] if c is not None and c[0] == x_used._version else None   # bf16x3: wgrad reuses the split
         ctx.wprep = getattr(w, "_gifb200_prep", None)
@@ -258,20 +261,37 @@ class _Conv(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gy):
-        x, w, x_arg = ctx.saved_tensors
-        k, mode, flip, transposed, in_hw, x_tf32 = ctx.cfg
+        x, w, x_arg, y = ctx.saved_tensors
+        k, mode, flip, transposed, in_hw, x_tf32, act, bias_shape = ctx.cfg
         _tag(x, x_tf32)
         _carry_planes(x, ctx.planes)
         if ctx.wprep is not None:
             w._gifb200_prep = ctx.wprep              # the input-gradient convolution reuses the staged-weight cache
-        gx = gw = None
+        gx = gw = gb = None
+        if act is not None:                          # gy becomes the gradient w.r.t. the pre-activation
+            slope, gain, _ = act
+            want_b = bias_shape is not None and ctx.needs_input_grad[2]
+            if not torch.is_grad_enabled():
+                # first-order backward: activation backward and bias gradient in one pass over (gy, y); in bf16x3 mode
+                # the pass writes the dgrad / wgrad operand (split planes) directly, no fp32 copy
+                gy = _c(gy)
+                C = gy.shape[-1]
+                carrier = C % 32 == 0 and _x3_backward_on_planes(x.shape, gy.shape, k, mode)
+                gy, _, gb, _ = _tail_bwd(gy, y, y, None, 1, gy.numel() // max(C, 1), C, slope, gain,
+                                         gt="planes" if carrier else "fp32", gb=want_b)
+            else:
+                gy = act_bwd(gy, y, slope, gain, rt=tf32_enabled())
+                if want_b and _WEIGHT_GRADS[0]:
+                    gb = rows_sum(gy.reshape(1, -1, gy.shape[-1]))
+            gb = None if gb is None else gb.reshape(bias_shape)
         if ctx.needs_input_grad[0]:
             # adj(S1, f, t) = (S1, !f, !t); adj(S2, f, t) = (T2, f, !t); adj(T2, f, t) = (S2, f, !t)
-            gx = _Conv.apply(gy, w, k, _ADJ_MODE[mode], (not flip) if mode == S1 else flip, not transposed, in_hw)
+            gx = _Conv.apply(gy, w, None, k, _ADJ_MODE[mode], (not flip) if mode == S1 else flip, not transposed, in_hw,
+                             None)
         if ctx.needs_input_grad[1] and _WEIGHT_GRADS[0]:
             xw = x_arg if x_arg is not None and torch.is_grad_enabled() else x
             gw = _ConvWgrad.apply(xw, gy, k, mode, flip, transposed)
-        return gx, gw, None, None, None, None, None
+        return gx, gw, gb, None, None, None, None, None, None
 
 
 class _ConvWgrad(torch.autograd.Function):
@@ -290,83 +310,25 @@ class _ConvWgrad(torch.autograd.Function):
         k, mode, flip, transposed = ctx.cfg
         gx = ggy = None
         if ctx.needs_input_grad[0]:   # <ggw, wgrad(x, gy)> = <gy, conv(x; ggw)>  ->  d/dx = adj conv of gy with ggw
-            gx = _Conv.apply(gy, ggw, k, _ADJ_MODE[mode], (not flip) if mode == S1 else flip, not transposed,
-                             tuple(x.shape[1:3]))
+            gx = _Conv.apply(gy, ggw, None, k, _ADJ_MODE[mode], (not flip) if mode == S1 else flip, not transposed,
+                             tuple(x.shape[1:3]), None)
         if ctx.needs_input_grad[1]:
-            ggy = _Conv.apply(x, ggw, k, mode, flip, transposed, tuple(gy.shape[1:3]))
+            ggy = _Conv.apply(x, ggw, None, k, mode, flip, transposed, tuple(gy.shape[1:3]), None)
         return gx, ggy, None, None, None, None
-
-
-class _ConvBiasAct(torch.autograd.Function):
-    """y = lrelu(conv(x; w) + bias, slope) * gain in ONE kernel (fused epilogue of gifb200_conv2d): ConvLayer =
-    EqualConv2d -> FusedLeakyReLU (cl.py:752-799), nn.Conv2d(+ReLU) of NoiseInjection (cl.py:405-414).  The backward is
-    composed of the differentiable primitives (activation backward from the saved OUTPUT, adjoint conv, wgrad)."""
-
-    @staticmethod
-    def forward(ctx, x_arg, w, bias, k, mode, slope, gain, rt, out_hw):
-        x, w = _c(x_arg), _c(w)
-        bias_flat = None if bias is None else _c(bias.reshape(-1))
-        y, x_used = _conv_raw(x, w, k, mode, False, False, out_hw, (bias_flat, slope, gain, rt))
-        ctx.save_for_backward(x_used, w, y, x_arg if x_used is not x and ctx.needs_input_grad[0] else None)   # as _Conv
-        ctx.cfg = (k, mode, slope, gain, tuple(x.shape[1:3]), _is_tf32(x_used), None if bias is None else bias.shape)
-        c = getattr(x_used, "_gifb200_planes", None)
-        ctx.planes = c[1] if c is not None and c[0] == x_used._version else None
-        ctx.wprep = getattr(w, "_gifb200_prep", None)
-        return y
-
-    @staticmethod
-    def backward(ctx, gy):
-        x, w, y, x_arg = ctx.saved_tensors
-        k, mode, slope, gain, in_hw, x_tf32, bias_shape = ctx.cfg
-        _tag(x, x_tf32)
-        _carry_planes(x, ctx.planes)
-        if ctx.wprep is not None:
-            w._gifb200_prep = ctx.wprep
-        gb = None
-        if not torch.is_grad_enabled():
-            # first-order backward: activation backward and bias gradient in one pass over (gy, y)
-            gy = _c(gy)
-            rt = tf32_enabled()
-            C = gy.shape[-1]
-            rows = gy.numel() // max(C, 1)
-            gt = torch.empty_like(gy)
-            want_b = bias_shape is not None and ctx.needs_input_grad[2]
-            gbf = torch.empty(C, dtype=torch.float32, device=gy.device) if want_b else None
-            if C % 32 == 0 and _x3_backward_on_planes(x.shape, gy.shape, k, mode):
-                # bf16x3: the activation backward writes the dgrad / wgrad operand (split planes) directly, no fp32 copy
-                pl = torch.empty((2,) + tuple(gy.shape), dtype=torch.bfloat16, device=gy.device)
-                check(lib.gifb200_tail_bwd_planes(ptr(gy), ptr(y), ptr(y), None, None, None, ptr(gbf), None, 1, rows, C, slope,
-                                                  gain, ptr(pl), None, stream()), "gifb200_tail_bwd_planes")
-                gt._gifb200_planes = (gt._version, pl)
-            else:
-                check(lib.gifb200_tail_bwd(ptr(gy), ptr(y), ptr(y), None, ptr(gt), None, ptr(gbf), None, 1, rows, C, slope, gain,
-                                           int(rt), stream()), "gifb200_tail_bwd")
-            _tag(gt, rt)
-            if want_b:
-                gb = gbf.reshape(bias_shape)
-        else:
-            gt = act_bwd(gy, y, slope, gain, rt=tf32_enabled())
-            if bias_shape is not None and ctx.needs_input_grad[2] and _WEIGHT_GRADS[0]:
-                gb = rows_sum(gt.reshape(1, -1, gt.shape[-1])).reshape(bias_shape)
-        gx = gw = None
-        if ctx.needs_input_grad[0]:
-            gx = _Conv.apply(gt, w, k, _ADJ_MODE[mode], mode == S1, True, in_hw)
-        if ctx.needs_input_grad[1] and _WEIGHT_GRADS[0]:
-            gw = _ConvWgrad.apply(x_arg if x_arg is not None and torch.is_grad_enabled() else x, gt, k, mode, False, False)
-        return gx, gw, gb, None, None, None, None, None, None
 
 
 def conv2d_bias_act(x, w, bias, k, mode=S1, slope=0.2, gain=math.sqrt(2.0), rt=False):
     """Fused conv + bias + leaky-ReLU*gain (slope=1, gain=1: plain bias add; slope=0: ReLU)."""
     hi, wi = x.shape[1:3]
     out_hw = (conv_out_size(hi, k, mode), conv_out_size(wi, k, mode))
-    return _tag(_ConvBiasAct.apply(x, w, bias, k, mode, float(slope), float(gain), bool(rt), out_hw), rt)
+    return _tag(_Conv.apply(x, w, bias, k, mode, False, False, out_hw, (float(slope), float(gain), bool(rt))), rt)
 
 
 def conv2d(x, w, k, mode=S1, flip=False, transposed=False):
     """x (B,H,W,Ci) NHWC, w (k*k, Co, Ci) tap-major [or (k*k, Ci, Co) with transposed=True] -> (B,Ho,Wo,Co)."""
     hi, wi = x.shape[1:3]
-    return _Conv.apply(x, w, k, mode, flip, transposed, (conv_out_size(hi, k, mode), conv_out_size(wi, k, mode)))
+    return _Conv.apply(x, w, None, k, mode, flip, transposed, (conv_out_size(hi, k, mode), conv_out_size(wi, k, mode)),
+                       None)
 
 
 _NO_WEIGHT_CACHE = False    # tests set this to compare against prepare-and-stage on every call (as cache=False)
@@ -486,6 +448,50 @@ def upfirdn2d(x, kernel, up=1, down=1, pad=(0, 0), rt=False):
 
 
 # --------------------------------------------------------------------------------------------- bias / act
+def _grad_planes(C, P):
+    """True when an elementwise gradient of C channels and P pixels per image goes on to bf16x3 tensor-core contractions:
+    its producer then writes the split planes in the same pass, which saves the split pass's read."""
+    return CONV_IMPL == 3 and C % 32 == 0 and P >= 256
+
+
+def _tail_bwd(gy, y, acc, d, B, P, C, slope, gain, gt=None, gacc=None, gb=False, gd=False):
+    """The fused first-order tail backward (gifb200_tail_bwd, or gifb200_tail_bwd_planes when any planes are wanted) on
+    contiguous tensors.  gt, gacc: None (not computed), "fp32", "both" (fp32 and planes) or "planes" (an unwritten fp32
+    tensor carrying the planes: only for the two tensor-core contractions of _x3_backward_on_planes); gb, gd: whether the
+    bias / modulation gradient is computed.  Returns (gt, gacc, gb (C,), gd (B, C)), None for what was not computed."""
+    outs = [None if m is None else torch.empty_like(gy) for m in (gt, gacc)]
+    gbt = torch.empty(C, dtype=torch.float32, device=gy.device) if gb else None
+    gdt = torch.empty((B, C), dtype=torch.float32, device=gy.device) if gd else None
+    fp32 = [t if m in ("fp32", "both") else None for t, m in zip(outs, (gt, gacc))]
+    planes = [torch.empty((2,) + tuple(gy.shape), dtype=torch.bfloat16, device=gy.device) if m in ("planes", "both")
+              else None for m in (gt, gacc)]
+    if planes[0] is not None or planes[1] is not None:
+        rt = False                                   # the planes entry point does not round its fp32 outputs
+        check(lib.gifb200_tail_bwd_planes(ptr(gy), ptr(y), ptr(acc), ptr(d), ptr(fp32[0]), ptr(fp32[1]), ptr(gbt), ptr(gdt),
+                                          B, P, C, slope, gain, ptr(planes[0]), ptr(planes[1]), stream()),
+              "gifb200_tail_bwd_planes")
+    else:
+        rt = tf32_enabled()
+        check(lib.gifb200_tail_bwd(ptr(gy), ptr(y), ptr(acc), ptr(d), ptr(fp32[0]), ptr(fp32[1]), ptr(gbt), ptr(gdt), B, P, C,
+                                   slope, gain, int(rt), stream()), "gifb200_tail_bwd")
+    for t, pl in zip(outs, planes):
+        if t is not None:
+            _carry_planes(t, pl)
+            _tag(t, rt)
+    return outs[0], outs[1], gbt, gdt
+
+
+def _scale_bwd(gy, x, s, rt=False):
+    """The fused first-order backward of y = x*s[b,c] (gifb200_scale_bwd) on contiguous tensors: (gx = gy*s, gs = sum_p gy*x);
+    rt: round gx to tf32."""
+    B, C = gy.shape[0], gy.shape[-1]
+    P = gy.numel() // max(B * C, 1)
+    gx = torch.empty_like(gy)
+    gs = torch.empty((B, C), dtype=torch.float32, device=gy.device)
+    check(lib.gifb200_scale_bwd(ptr(gy), ptr(x), ptr(s), ptr(gx), ptr(gs), B, P, C, int(rt), stream()), "gifb200_scale_bwd")
+    return _tag(gx, rt), gs
+
+
 class _BiasAct(torch.autograd.Function):
     """y = lrelu(x*rowscale[b,c] + add + bias[c], slope) * gain  (rowscale/add/bias optional)."""
 
@@ -512,32 +518,15 @@ class _BiasAct(torch.autograd.Function):
         if not torch.is_grad_enabled():
             # first-order backward only (no create_graph): one fused pass instead of act_bwd + chan_scale + spatial_dot + rows_sum
             gy = _c(gy)
-            rt = tf32_enabled()
             B, C = gy.shape[0], gy.shape[-1]
             P = gy.numel() // max(B * C, 1)
-            gt = torch.empty_like(gy)
-            gacc = torch.empty_like(gy) if rowscale is not None else None
             want_b = bias_shape is not None and ctx.needs_input_grad[3]
-            want_d = rowscale is not None and ctx.needs_input_grad[1]
-            gb = torch.empty(C, dtype=torch.float32, device=gy.device) if want_b else None
-            gd = torch.empty((B, C), dtype=torch.float32, device=gy.device) if want_d else None
-            if CONV_IMPL == 3 and C % 32 == 0 and P >= 256:
-                # bf16x3: the gradients leave on autograd edges towards convolutions (the modulated conv and the noise branch)
-                # or FIR filters: write the fp32 form AND the split planes in the same pass (saves the split pass's read)
-                pt = torch.empty((2,) + tuple(gy.shape), dtype=torch.bfloat16, device=gy.device) if has_add else None
-                pa = torch.empty((2,) + tuple(gy.shape), dtype=torch.bfloat16, device=gy.device) if gacc is not None else None
-                check(lib.gifb200_tail_bwd_planes(ptr(gy), ptr(y), ptr(x), ptr(rowscale), ptr(gt), ptr(gacc), ptr(gb), ptr(gd), B,
-                                                  P, C, slope, gain, ptr(pt), ptr(pa), stream()), "gifb200_tail_bwd_planes")
-                if pt is not None:
-                    gt._gifb200_planes = (gt._version, pt)
-                if pa is not None:
-                    gacc._gifb200_planes = (gacc._version, pa)
-            else:
-                check(lib.gifb200_tail_bwd(ptr(gy), ptr(y), ptr(x), ptr(rowscale), ptr(gt), ptr(gacc), ptr(gb), ptr(gd), B, P, C,
-                                           slope, gain, int(rt), stream()), "gifb200_tail_bwd")
-            _tag(gt, rt)
-            if gacc is not None:
-                _tag(gacc, rt)
+            # bf16x3: the gradients leave on autograd edges towards convolutions (the modulated conv and the noise branch)
+            # or FIR filters: write the fp32 form AND the split planes in the same pass
+            x3 = _grad_planes(C, P)
+            gt, gacc, gb, gd = _tail_bwd(gy, y, x, rowscale, B, P, C, slope, gain, gt="both" if x3 and has_add else "fp32",
+                                         gacc=None if rowscale is None else ("both" if x3 else "fp32"), gb=want_b,
+                                         gd=rowscale is not None and ctx.needs_input_grad[1])
             gx = (gacc if rowscale is not None else gt) if ctx.needs_input_grad[0] else None
             return (gx, gd, gt if (has_add and ctx.needs_input_grad[2]) else None,
                     gb.reshape(bias_shape) if want_b else None, None, None, None)
@@ -571,24 +560,14 @@ class _TailBwdCG(torch.autograd.Function):
     def forward(ctx, gy, y, acc, d, slope, gain, want_planes):
         gy, acc, d = _c(gy), _c(acc), _c(d)
         require_cuda(gy, acc, d)
-        B, C = gy.shape[0], gy.shape[-1]
-        P = gy.numel() // max(B * C, 1)
-        gacc = torch.empty_like(gy)
-        gd = torch.empty((B, C), dtype=torch.float32, device=gy.device)
         if y is None:
-            check(lib.gifb200_scale_bwd(ptr(gy), ptr(acc), ptr(d), ptr(gacc), ptr(gd), B, P, C, 0, stream()), "gifb200_scale_bwd")
+            gacc, gd = _scale_bwd(gy, acc, d)
         else:
             y = _c(y)
-            if want_planes and CONV_IMPL == 3 and C % 32 == 0 and P >= 256:
-                pa = torch.empty((2,) + tuple(gy.shape), dtype=torch.bfloat16, device=gy.device)
-                check(lib.gifb200_tail_bwd_planes(ptr(gy), ptr(y), ptr(acc), ptr(d), None, ptr(gacc), None, ptr(gd), B, P, C,
-                                                  slope, gain, None, ptr(pa), stream()), "gifb200_tail_bwd_planes")
-                gacc._gifb200_planes = (gacc._version, pa)
-            else:
-                rt = tf32_enabled()
-                check(lib.gifb200_tail_bwd(ptr(gy), ptr(y), ptr(acc), ptr(d), None, ptr(gacc), None, ptr(gd), B, P, C, slope, gain,
-                                           int(rt), stream()), "gifb200_tail_bwd")
-                _tag(gacc, rt)
+            B, C = gy.shape[0], gy.shape[-1]
+            P = gy.numel() // max(B * C, 1)
+            _, gacc, _, gd = _tail_bwd(gy, y, acc, d, B, P, C, slope, gain,
+                                       gacc="both" if want_planes and _grad_planes(C, P) else "fp32", gd=True)
         ctx.save_for_backward(gy, y, acc, d)
         ctx.cfg = (slope, gain, y is not None)
         ctx.set_materialize_grads(False)
@@ -609,12 +588,11 @@ class _TailBwdCG(torch.autograd.Function):
         gx2 = torch.empty_like(gy) if (ctx.needs_input_grad[2] and ggd is not None) else None
         gdd = torch.empty((B, C), dtype=torch.float32, device=gy.device) if (ctx.needs_input_grad[3] and gg is not None) else None
         pp = None
-        if ggy is not None and not has_y and CONV_IMPL == 3 and C % 32 == 0 and P >= 256:
+        if ggy is not None and not has_y and _grad_planes(C, P):
             pp = torch.empty((2,) + tuple(gy.shape), dtype=torch.bfloat16, device=gy.device)   # gy came out of a convolution
         check(lib.gifb200_tail_bwd2(ptr(gg), ptr(ggd), ptr(gy), ptr(y) if has_y else None, ptr(acc), ptr(d), ptr(ggy), ptr(gx2),
                                     ptr(gdd), B, P, C, slope, gain, ptr(pp), stream()), "gifb200_tail_bwd2")
-        if pp is not None:
-            ggy._gifb200_planes = (ggy._version, pp)
+        _carry_planes(ggy, pp)
         return ggy, None, gx2, gdd, None, None, None
 
 
@@ -689,15 +667,8 @@ class _ChanScale(torch.autograd.Function):
     def backward(ctx, gy):
         x, s = ctx.saved_tensors
         if not torch.is_grad_enabled() and ctx.needs_input_grad[0] and ctx.needs_input_grad[1]:
-            gy = _c(gy)                                    # fused first-order pass: gx = gy*s, gs = sum gy*x
-            rt = tf32_enabled()
-            B, C = gy.shape[0], gy.shape[-1]
-            P = gy.numel() // max(B * C, 1)
-            gx = torch.empty_like(gy)
-            gs = torch.empty((B, C), dtype=torch.float32, device=gy.device)
-            check(lib.gifb200_scale_bwd(ptr(gy), ptr(x), ptr(s), ptr(gx), ptr(gs), B, P, C, int(rt), stream()),
-                  "gifb200_scale_bwd")
-            return _tag(gx, rt), gs, None
+            gx, gs = _scale_bwd(_c(gy), x, s, tf32_enabled())     # fused first-order pass: gx = gy*s, gs = sum gy*x
+            return gx, gs, None
         if torch.is_grad_enabled() and not _WEIGHT_GRADS[0] and ctx.needs_input_grad[0] and ctx.needs_input_grad[1]:
             gx, gs = _TailBwdCG.apply(gy, None, x, s, 1.0, 1.0, False)     # one node, fused second-order rule
             return gx, gs, None
@@ -760,7 +731,7 @@ class _ModConvX3(torch.autograd.Function):
         k, mode, in_hw = ctx.cfg
         if ctx.wprep is not None:
             w._gifb200_prep = ctx.wprep
-        adj = (gy, w, k, _ADJ_MODE[mode], mode == S1, True, in_hw)
+        adj = (gy, w, None, k, _ADJ_MODE[mode], mode == S1, True, in_hw, None)
         if torch.is_grad_enabled():
             gxs = _Conv.apply(*adj) if (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]) else None
             if not _WEIGHT_GRADS[0] and gxs is not None:
@@ -776,11 +747,7 @@ class _ModConvX3(torch.autograd.Function):
         gx = gs = gw = None
         if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
             gxs, _ = _conv_raw(gy, w, k, _ADJ_MODE[mode], mode == S1, True, in_hw)
-            B, C = gxs.shape[0], gxs.shape[-1]
-            P = gxs.numel() // max(B * C, 1)
-            gx = torch.empty_like(gxs)
-            gs = torch.empty((B, C), dtype=torch.float32, device=gy.device)
-            check(lib.gifb200_scale_bwd(ptr(gxs), ptr(x), ptr(s), ptr(gx), ptr(gs), B, P, C, 0, stream()), "gifb200_scale_bwd")
+            gx, gs = _scale_bwd(gxs, x, s)
         if ctx.needs_input_grad[2] and _WEIGHT_GRADS[0]:
             gw = _wgrad_raw(x, gy, k, mode, False, False, x_planes=ctx.planes)
         return gx, gs, gw, None, None, None
@@ -1087,11 +1054,7 @@ def conv2d_ex(x, w, kh, kw, stride=1, pad=(0, 0), bias=None, relu=False, out=Non
     elif out.shape[:3] != (B, Ho, Wo) or not out.is_contiguous() or out.dtype != torch.float32:
         raise ValueError(f"conv2d_ex: out {tuple(out.shape)} is not a contiguous (B, {Ho}, {Wo}, Cy) float32 tensor")
     impl = conv2d_ex_impl(x.shape, Co, kh, kw, stride, pad)
-    xin = x
-    if impl == 3:
-        xin = _planes(x)
-    elif impl == 2 and not _is_tf32(x):
-        xin = _tag(_round_tf32_raw(x), True)
+    xin = _tc_operand(x, impl)
     nws = lib.gifb200_conv2d_ex_workspace_bytes(B, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad[0], pad[1], impl)
     flag = 0
     if nws == 0:

@@ -60,7 +60,8 @@ SHAPES = [(2, 256, 32), (2, 300, 64), (1, 289, 512), (2, 256, 512)]     # P >= 2
 @pytest.mark.parametrize("B,P,C", SHAPES)
 @pytest.mark.parametrize("want_b", [False, True])
 def test_tail_bwd_planes_conv_bias_act(cuda, B, P, C, want_b):
-    """_ConvBiasAct's first-order backward: only the planes of gt (no fp32 gt), acc = y, no d, optional bias gradient."""
+    """The first-order backward of _Conv's fused epilogue: only the planes of gt (no fp32 gt), acc = y, no d, optional
+    bias gradient."""
     ops = _ops()
     rows, slope, gain = B * P, 0.2, 2 ** 0.5
     gy, y = _rand((rows, C), 1), _rand((rows, C), 2)

@@ -3,10 +3,10 @@ against float64 torch references.
 
 The training step differentiates its own backward twice: R1 (d scores / d image inside ``ops.input_gradient_only()``,
 then the weight gradient of its square norm) and the path-length term (d image / d w, then its gradient).  Those passes
-run branches of gif_b200.ops that no first-order test reaches: the grad-enabled backwards of _Conv, _ConvWgrad,
-_ConvBiasAct and _ModConvX3, the fused second-order node _TailBwdCG with its bf16x3 planes, _ActBwd / spatial_dot /
-chan_scale as differentiable nodes, and weight gradients of input-gradient convolutions, (flip, transposed) = (True, True)
-for S1 and (False, True) for T2 / S2.
+run branches of gif_b200.ops that no first-order test reaches: the grad-enabled backwards of _Conv (with and without its
+fused epilogue), _ConvWgrad and _ModConvX3, the fused second-order node _TailBwdCG with its bf16x3 planes, _ActBwd /
+spatial_dot / chan_scale as differentiable nodes, and weight gradients of input-gradient convolutions, (flip, transposed)
+= (True, True) for S1 and (False, True) for T2 / S2.
 
 References: float64 torch with the physical weight mapping of gifb200.h, and the leaky-ReLU masks taken from the CUDA
 forward output, m = where(y > 0, 1, slope) * gain (what act_bwd / tail_bwd use).  Every reference is then linear in the
